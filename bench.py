@@ -10,13 +10,15 @@ layers and the whole UNet), gradient all-reduce (N > 1), global-norm clip + Adam
     e2e   = same through DreamLLMForCausalMLM.forward/backward with pinned HOST ids + images (12.6 MB H2D / step) and loss D2H
 
 Nested records in the same JSON line, each with its own roofline:
-    c2  configs[1]  Vicuna-7B text-only fwd+bwd, seq 2048, bs 8 / GPU  (tcgen05 GEMM roofline + whole-step tensor fraction; DDP at N > 1)
+    c2  configs[1]  Vicuna-7B text-only fwd+bwd, seq 2048, bs 4 / GPU  (GEMM roofline + whole-step tensor fraction; DDP at N > 1;
+                    bs 4 keeps weights, gradients and activations inside an 80 GB H100)
     c4  configs[3]  SD-2.1 UNet 64x64, 50-step DDIM, 77 dream-query embeddings, bs 16, CFG, whole loop in ONE CUDA graph
                     (step tensor fraction + per-kernel HBM fractions of GroupNorm / LayerNorm / GEGLU / sampler)
     c3  configs[2]  CLIP ViT-L/14-336 + linear projector + Vicuna-7B, 576 visual + 1024 text tokens, bs 4, fwd+bwd through the collator
     c1  configs[0]  one DreamLLMDecoderLayer fwd+bwd, hidden 4096 seq 512 bs 1, with the CPU reference timed in full beside it
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path (N>1 under torchrun, weak scaling)
+  python bench.py ... --dump-outputs DIR                   # + the headline step's outputs of its last timed step as DIR/<name>.npy
   python bench.py --impl reference ...                     # the reference algorithm on the host CPU cores (oracle port), same workload
 
 One JSON line on stdout (rank 0).
@@ -37,7 +39,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "interleaved tokens+pixels/sec @ Vicuna-7B+SD2.1 512px, 1/2/4/8 B200"
+METRIC = "interleaved tokens+pixels/sec @ Vicuna-7B+SD2.1 512px, 1/2/4/8 H100"
 UNIT = "tokens+pixels/s"
 BF = torch.bfloat16
 
@@ -64,7 +66,7 @@ def c5_flops_per_gpu(bs, seq):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -128,9 +130,9 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"tf_sustained": d.get("bf16_tflops_sustained", 1442.3), "tf_burst": d.get("bf16_tflops", 1701.0),
-                "hbm": d.get("hbm_gbs", 6569.6), "how": "measured (MEASURED_PEAKS.json)"}
-    return {"tf_sustained": 1400.0, "tf_burst": 1590.0, "hbm": 6650.0, "how": "fallback (B200_PROFILING.md)"}
+        return {"tf_sustained": float(d["bf16_tflops_sustained"]), "tf_burst": float(d["bf16_tflops"]), "hbm": float(d["hbm_gbs"]),
+                "how": "measured (MEASURED_PEAKS.json)"}
+    return {"tf_sustained": 989.0, "tf_burst": 989.0, "hbm": 3350.0, "how": "H100 SXM data sheet (dense bf16, HBM3), not measured"}
 
 
 def gemm_traffic():
@@ -382,6 +384,7 @@ def run_c5(env, model, steps, warmup):
     from dreamllm_b200.modeling_plugins import DreamEmbedding, StableDiffusionHead, build_splice_plan
     dev, world, rank, dist = env.dev, env.world, env.rank, env.dist
     B, Q, TXT, R = C5["bs"], C5["Q"], C5["txt"], C5["res"]
+    torch.manual_seed(4321)                                       # same plugin weights whichever records ran before
     old = torch.get_default_dtype()
     torch.set_default_dtype(BF)
     with torch.device(dev):
@@ -497,6 +500,9 @@ def run_c5(env, model, steps, warmup):
                     "h2d_bytes_per_step": int(ids_pin.numel() * 8 + imgs.numel() * 4), "d2h_bytes_per_step": 4},
             "launches_per_step": launches_per_step, "launch_mode": mode, "vm_loss": float(loss_static.item()) / model.loss_weight_vm,
             "trainable_params": n_tr,
+            # what a training loop receives from the last timed step: its loss, the trainable gradients, the parameters after AdamW
+            "_outputs": {"loss": loss_static.float().cpu(), "trainable_grads": flat_g[:n_tr].float().cpu(),
+                         "trainable_params": flat_p[:n_tr].float().cpu()},
             "roofline": {"bound": "tensor", "scope": "whole step (LLM fwd+dgrad, VAE encode, UNet fwd+dgrad)",
                          "algorithmic_tflop_per_step_per_gpu": fl / 1e12, "achieved": fl / 1e12 / (ms / 1e3), "peak": env.peaks["tf_sustained"],
                          "unit": "TFLOP/s", "frac": fl / 1e12 / (ms / 1e3) / env.peaks["tf_sustained"],
@@ -557,14 +563,14 @@ def run_c2(env, model, steps, warmup, bs, seq, layers):
             "ms_per_step": ms, "tokens_per_s": toks / ms * 1e3, "e2e_tokens_per_s": toks / ms_e * 1e3,
             "h2d_bytes_per_step": int(host_ids.numel() * 8), "d2h_bytes_per_step": 4, "gpu_launches": launches,
             "ddp": None if world == 1 else {"bucket_mb": 512, "grad_bytes": 2 * sum(p.numel() for p in params), "grad_copies_into_buckets": copies},
-            "roofline": {"bound": "tensor", "kernel": "dllm::gemm_kernel<2,*,*,bf16> (tcgen05 GEMM, all fwd/dgrad/wgrad launches)",
+            "roofline": {"bound": "tensor", "kernel": "dllm::gemm_kernel<*,*,bf16> (wgmma GEMM, all fwd/dgrad/wgrad launches)",
                          "achieved": gs["tflops"], "peak": pk["tf_sustained"], "unit": "TFLOP/s",
                          "frac": gs["tflops"] / pk["tf_sustained"] if gs["tflops"] else None, "traffic": gemm_traffic()[0],
                          "traffic_note": gemm_traffic()[1], "peak_source": f"bf16_tflops_sustained, {pk['how']}",
                          "launches_timed": gs["n"], "gemm_share_of_step": gs["ms"] / total if total else None},
             "step_roofline": {"algorithmic_tflop_per_step_per_gpu": fl / 1e12, "achieved_tflops_per_gpu": fl / 1e12 / (ms / 1e3),
-                              "frac_of_measured_sustained_peak": fl / 1e12 / (ms / 1e3) / pk["tf_sustained"],
-                              "frac_of_measured_burst_peak": fl / 1e12 / (ms / 1e3) / pk["tf_burst"]}}
+                              "frac_of_sustained_peak": fl / 1e12 / (ms / 1e3) / pk["tf_sustained"],
+                              "frac_of_burst_peak": fl / 1e12 / (ms / 1e3) / pk["tf_burst"], "peak_source": pk["how"]}}
 
 
 def hbm_kernel_fracs(env):
@@ -749,22 +755,28 @@ def run_c1(env, model):
             "gpu_ms_eager": ms_eager, "launch_mode": "fwd+bwd captured in one CUDA graph (median of 5 x 20 replays); eager median beside it",
             "roofline": {"bound": "tensor", "achieved": fl / 1e12 / (ms / 1e3), "peak": env.peaks["tf_burst"], "unit": "TFLOP/s",
                          "frac": fl / 1e12 / (ms / 1e3) / env.peaks["tf_burst"],
-                         "note": "M = 512: the 512 x 4096 outputs are 64 tiles on 148 SMs (< 1/2 wave) — latency-, not tensor-bound (SURVEY §7)"}}
+                         "note": "M = 512: the 512 x 4096 outputs are 64 tiles on 132 SMs (< 1/2 wave) — latency-, not tensor-bound (SURVEY §7)"}}
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5,
+                    help="timed steps of every GPU record (c4: timed 50-step denoising loops; c1 times its own fixed batches); "
+                         "the CPU reference arm times min(steps, 3)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--layers", type=int, default=L, help="dev only: fewer layers (reported in config; not a valid bench)")
-    ap.add_argument("--bs", type=int, default=8, help="c2 batch per GPU")
+    ap.add_argument("--bs", type=int, default=4, help="c2 batch per GPU")
     ap.add_argument("--seq", type=int, default=2048, help="c2 sequence length")
     ap.add_argument("--only", default="", help="dev only: comma list of records to run (c5,c2,c4,c3,c1)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--fast", action="store_true", help="skip the slow CPU legs (c1 in full, c2 sample)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the headline step's outputs of its last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     rank = int(os.environ.get("RANK", 0))
 
     if args.impl == "reference":
@@ -785,9 +797,9 @@ def main():
     # order: c1 / c2 / c3 need every LLM weight trainable; c5 re-freezes the LLM, so it runs after them; c4 is independent
     for name, fn in (("c1", lambda: run_c1(env, model)),
                      ("c2", lambda: run_c2(env, model, args.steps, args.warmup, args.bs, args.seq, args.layers)),
-                     ("c3", lambda: run_c3(env, model, min(args.steps, 3), 2)),
+                     ("c3", lambda: run_c3(env, model, args.steps, 2)),
                      ("c5", lambda: run_c5(env, model, args.steps, args.warmup)),
-                     ("c4", lambda: run_c4(env))):
+                     ("c4", lambda: run_c4(env, runs=args.steps))):
         if name not in only:
             continue
         lo = sampler.mark()
@@ -809,6 +821,13 @@ def main():
         return
 
     c5 = rec.get("c5")
+    outputs = c5.pop("_outputs") if c5 is not None else {}
+    if args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in outputs.items():
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), v.numpy().astype(np.float32))
+        log(f"outputs of the last timed c5 step written to {args.dump_outputs}: {sorted(outputs)}")
     head_rec = c5 if c5 is not None else next(iter(rec.values()))
     line = {"metric": METRIC, "value": head_rec.get("value"), "unit": UNIT, "n_gpus": env.world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": head_rec.get("ms_per_step"), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
@@ -820,7 +839,7 @@ def main():
         line["gpu_launches"] = int(c5["launches_per_step"] * args.steps * 2)       # timed device-resident + e2e regions
         line["launch_mode"] = c5["launch_mode"]
         line["step_roofline"] = c5["roofline"]
-    # the dominant kernel of the path is the tcgen05 GEMM; its live-event roofline comes from the c2 record (large-M launches)
+    # the dominant kernel of the path is the wgmma GEMM; its live-event roofline comes from the c2 record (large-M launches)
     if "c2" in rec and "roofline" in rec["c2"]:
         line["roofline"] = rec["c2"]["roofline"]
     elif c5 is not None:

@@ -11,9 +11,9 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.environ.get("DLLM_LIB_PATH") or os.path.join(_HERE, "libdreamllm_sm100.so")   # env override: A/B builds in dev scripts
-SOURCES = ["capi.cu", "gemm_sm100.cu", "elementwise.cu", "attn_sm100.cu", "unet_ops.cu", "optim.cu"]
+SOURCES = ["capi.cu", "gemm_sm90.cu", "elementwise.cu", "attn_sm90.cu", "unet_ops.cu", "optim.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
 ]
 
@@ -27,7 +27,7 @@ def _needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """nvcc-compile every .cu for sm_100a into dreamllm_b200/libdreamllm_sm100.so (in-tree, travels with gpurun)."""
+    """nvcc-compile every .cu for sm_90a into dreamllm_b200/libdreamllm_sm100.so (in-tree, next to this module)."""
     if not force and not _needs_build():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -50,7 +50,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed for {src}:\n{out}")
         if verbose and out:
             print(out)
-    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if out.returncode != 0:
         raise RuntimeError(f"link failed:\n{out.stdout}")
@@ -109,7 +109,6 @@ SIGNATURES = {
     "dllm_timestep_embedding_batch": (_i, [_vp, _vp, _i, _i, _vp]),
     "dllm_sampler_step": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _l, _vp]),
     "dllm_attn_bwd_ex": (_i, [_vp] * 11 + [_sz, _i, _i, _i, _i, _i, _l, _l, _l, _l, _l, _i, _f, _vp]),
-    "dllm_attn_item_order": (None, [_i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "dllm_groupnorm_stats": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _i, _f, _vp]),
     "dllm_groupnorm_apply": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "dllm_groupnorm_bwd_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _i, _vp]),

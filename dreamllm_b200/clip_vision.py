@@ -1,4 +1,4 @@
-"""B200-native CLIP ViT vision tower (forward only), state-dict compatible with `transformers.CLIPVisionModel`.
+"""H100-native CLIP ViT vision tower (forward only), state-dict compatible with `transformers.CLIPVisionModel`.
 
 Reference call site: `CLIPVisionEmbedding.forward`, modeling_plugins.py:321-323 —
     output = self.clip_vision_model(images, output_hidden_states=True); hidden_states[select_layer][:, 1:]
@@ -6,7 +6,7 @@ The arithmetic lives in transformers==4.35.2 `modeling_clip.py` (CLIPVisionEmbed
 CLIPMLP), restated per SURVEY.md Appendix A.4: conv patch-embed (k=s=patch, no bias) + CLS + learned pos-emb ->
 pre_layrnorm -> L x { x += out_proj(attn(LN1 x)) ; x += fc2(quick_gelu(fc1(LN2 x))) }.
 
-Kernels: patch-embed = unfold + tcgen05 GEMM; fused q|k|v GEMM (+bias); non-causal tcgen05 flash attention d=64;
+Kernels: patch-embed = unfold + wgmma GEMM; fused q|k|v GEMM (+bias); non-causal wgmma flash attention d=64;
 out_proj / fc2 GEMMs with bias+residual epilogue; fc1 GEMM with bias+quick_gelu epilogue; LayerNorm kernel.
 Layers after `select_layer` are never computed (the reference runs and discards them, SURVEY §8 row a11).
 The tower is frozen on this path (freeze_clip_vision_model=True, configs/common.py:35) -> runs under no_grad.

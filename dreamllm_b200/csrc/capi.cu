@@ -1,13 +1,13 @@
 // extern "C" boundary of libdreamllm_sm100.so — see include/dreamllm_sm100.h for the contract.
 #include "../../include/dreamllm_sm100.h"
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 #include "ops.h"
 
 using namespace dllm;
 
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 
-// Autograd may call us on a worker thread that has never touched CUDA (observed on B200: cuTensorMapEncodeTiled ->
+// Autograd may call us on a worker thread that has never touched CUDA (observed: cuTensorMapEncodeTiled ->
 // CUDA_ERROR_INVALID_CONTEXT when the first CUDA work of the engine's device thread is one of our Functions).  Bind the
 // context that owns the caller's buffer — never "device 0" — before any driver/runtime call.
 typedef CUresult (*PFN_ctxGetCurrent)(CUcontext*);
@@ -239,9 +239,6 @@ int dllm_attn_bwd_ex(const void* dout, const void* q, const void* k, const void*
   ensure_context(dout);
   return attn_bwd_ex(dout, q, k, v, out, lse, dq, dk, dv, seqlens, workspace, workspace_bytes, B, Sq, Skv, nh, d, ld_q, ld_kv, ld_o,
                      ld_dq, ld_dkv, causal, scale, S(stream));
-}
-void dllm_attn_item_order(int w, int ntiles, int n_hb, int grid, int descending, int* tile, int* hb, int* win_heads) {
-  attn_item_order(w, ntiles, n_hb, grid, descending, tile, hb, win_heads);
 }
 int dllm_groupnorm_stats(const void* x, float* stats, void* workspace, size_t ws_bytes, int N, int HW, int C, int G, float eps, void* stream) {
   ensure_context(x);

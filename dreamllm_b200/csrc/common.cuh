@@ -1,6 +1,6 @@
-// Shared sm_100a device helpers: mbarrier, TMA, tcgen05/TMEM wrappers (raw PTX).
+// Shared sm_90a device helpers: mbarrier, TMA, wgmma wrappers (raw PTX).
 // Everything here is hand-written for this repo; encodings follow the PTX ISA / the public
-// CUTLASS headers' documentation of the UMMA descriptors.
+// CUTLASS headers' documentation of the GMMA descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -20,11 +20,6 @@ typedef __nv_bfloat16 bf16;
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -33,15 +28,6 @@ __device__ __forceinline__ bool elect_one_sync() {
       "selp.u32 %0, 1, 0, px;\n\t}"
       : "=r"(pred));
   return pred != 0;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same offset in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -60,10 +46,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// arrive on a barrier living in another CTA of the cluster (addr from mapa_shared)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -75,46 +57,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// cluster-scope acquire: pairs with a remote CTA's st.shared::cluster + mbarrier.arrive.release.cluster
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity, int tag = 0) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  long long t0 = clock64();
-  uint32_t spins = 0;
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if ((++spins & 0xfff) == 0 && clock64() - t0 > 4000000000LL) {
-      printf("dllm watchdog: cluster mbarrier wait timed out (tag %d, block %d, thread %d, parity %u)\n", tag, (int)blockIdx.x,
-             (int)threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void st_shared_cluster_u32(uint32_t cluster_addr, uint32_t v) {
-  asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
-}
+// Bounded wait (DLLM_WATCHDOG=1, the default): a protocol bug traps after ~2 s instead of hanging the GPU.  The slow path holds no
+// function call (no printf): ptxas serialises every wgmma of a kernel whose wgmma pipeline crosses a call (C7510), and the consumers
+// wait on the operand ring while their previous K block's wgmma group is still in flight.  `tag` names the wait site in the SASS
+// (the immediate of the trap's preceding move) for reading a core dump; it costs nothing at run time.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
 #if DLLM_WATCHDOG
   if (mbar_try_wait(bar, parity)) return;
-  long long t0 = clock64();
+  const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if ((++spins & 0xfff) == 0 && clock64() - t0 > 4000000000LL) {  // ~2 s
-      printf("dllm watchdog: mbarrier wait timed out (tag %d, block %d, thread %d, parity %u)\n", tag,
-             (int)blockIdx.x, (int)threadIdx.x, parity);
-      __trap();
+      asm volatile("{\n\t.reg .b32 t;\n\tmov.b32 t, %0;\n\ttrap;\n\t}" ::"r"(tag));
     }
   }
 #else
+  (void)tag;
   while (!mbar_try_wait(bar, parity)) {
   }
 #endif
@@ -130,16 +88,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
           smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-// 2-CTA flavour: data lands in this CTA's smem, the byte count is signalled on the barrier whose
-// shared::cluster address is given (the leader CTA's full barrier)
-__device__ __forceinline__ void tma_load_2d_2cta(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
       : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
@@ -159,149 +107,44 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-template <int kCta>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  if constexpr (kCta == 1)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-template <int kCta>
-__device__ __forceinline__ void tmem_relinquish() {
-  if constexpr (kCta == 1)
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  else
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCta>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCta == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread
-template <int kCta>
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (kCta == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M on the 128 lanes, two bf16 K-elements per 32-bit column, 8 columns per
-// UMMA_K = 16) is read straight from tensor memory — used by the attention kernels to feed P / dS from the softmax warps to the next
-// tile-GEMM without a round trip through shared memory.  A from TMEM is always K-major (idesc a_mn = 0).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// make all previously issued MMAs arrive on an mbarrier when they retire (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 2-CTA: arrive on the barrier at this smem offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread t gets lane base+t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// 16-column flavours (attention backward: 16 row warps split a 64-column tile four ways)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type 2), descriptor version 1 (Blackwell).
+// ----------------------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor of the sm_90 GMMA, 128-byte swizzle (layout type 1):
 //   bits [0,14)  start address >> 4       bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4  bits [46,48) version = 1     bits [61,64) layout type
+//   bits [32,46) stride byte offset >> 4  bits [62,64) layout type
 // K-major operand (rows x 64 bf16 per 128-byte line, 8-row swizzle atoms of 1024 B):
-//   SBO = 1024 (distance between 8-row groups); LBO unused (1).  Advance 32 B per UMMA_K=16.
+//   SBO = 1024 (distance between 8-row groups); LBO unused (16).  Advance 32 B per K = 16 step.
 // MN-major operand (64 mn-elements per 128-byte line, one line per k; boxes of [64 mn x BK k]):
-//   LBO = distance between 64-element mn groups (box bytes); SBO = 1024 (8 k-lines). Advance 2048 B per UMMA_K.
+//   LBO = distance between 64-element mn groups (box bytes); SBO = 1024 (8 k-lines).  Advance 2048 B per K = 16 step.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt  bit 15 A major (1 = MN)  bit 16 B major
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+// descriptor of K step `ks` (16 elements) of a 128B-swizzled tile
+//   K-major : tile = [K/64 chunks][rows][128 B]; chunk_stride = bytes between 64-wide K chunks
+//   MN-major: tile = [MN/64 groups][K lines][128 B]; chunk_stride = bytes between 64-wide MN groups (LBO)
+__device__ __forceinline__ uint64_t op_desc(uint32_t base, bool mn, uint32_t chunk_stride, int ks) {
+  return mn ? make_smem_desc(base + ks * 2048u, chunk_stride, 1024u)
+            : make_smem_desc(base + (ks >> 2) * chunk_stride + (ks & 3) * 32u, 16u, 1024u);
+}
+// wgmma_fence orders this warpgroup's register writes of accumulators / A fragments before the next wgmma reads them
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// per-warpgroup register budget (the TMA warpgroup hands registers to the MMA warpgroups)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // The 8-element vector copies of the HBM-bound kernels are 128-bit accesses, which fault on addresses that are not 16-byte aligned:
@@ -353,20 +196,5 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
           smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1,
-                                                 int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// Operand descriptor for one UMMA_K (=16) step `ks` of a 128B-swizzled smem tile.
-//   K-major : tile = [K/64 chunks][rows][128 B]; chunk_stride = bytes between 64-wide K chunks
-//   MN-major: tile = [MN/64 groups][K lines][128 B]; chunk_stride = bytes between 64-wide MN groups (LBO)
-__device__ __forceinline__ uint64_t op_desc(uint32_t base, bool mn, uint32_t chunk_stride, int ks) {
-  return mn ? make_smem_desc(base + ks * 2048u, chunk_stride, 1024u)
-            : make_smem_desc(base + (ks >> 2) * chunk_stride + (ks & 3) * 32u, 16u, 1024u);
 }
 }  // namespace dllm

@@ -1,10 +1,10 @@
-// HBM-bound kernels of the DreamLLM decoder path (sm_100a): RMSNorm fwd/bwd (+fused residual add),
+// HBM-bound kernels of the DreamLLM decoder path (sm_90a): RMSNorm fwd/bwd (+fused residual add),
 // RoPE (in place on the fused qkv buffer), SwiGLU fwd/bwd, shifted masked cross-entropy (fwd + in-place
 // dlogits), embedding gather / sorted segment scatter, bf16 add.
 // All move 8-element (16-byte) vectors per thread (128-bit LDG/STG, see the Vec8 note below), fp32 math, warp-shuffle reductions; rounding points follow the
 // reference's bf16 eager path (cited per kernel) so bf16-vs-bf16 parity holds to the last place where cheap.
 #include "common.cuh"
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 
 namespace dllm {
 
@@ -23,7 +23,7 @@ struct alignas(16) Vec8 {
     if (i == 0) u.x = w; else if (i == 1) u.y = w; else if (i == 2) u.z = w; else u.w = w;
   }
 };
-__device__ __forceinline__ void unpack8(const Vec8& p, float* f) {
+__device__ __forceinline__ void unpack8(const Vec8 p, float* f) {   // by value: one 128-bit load per vector
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     float2 t = __bfloat1622float2(p.get(i));
@@ -246,8 +246,9 @@ __global__ void rope_kernel(bf16* __restrict__ buf, const bf16* __restrict__ cos
   const int p = pos[t];
   bf16* base = buf + static_cast<size_t>(t) * ld + static_cast<size_t>(head) * D + vi * 8;
   float a[8], b[8], c1[8], c2[8], s1[8], s2[8];
-  unpack8(*reinterpret_cast<const Vec8*>(base), a);
-  unpack8(*reinterpret_cast<const Vec8*>(base + D / 2), b);
+  const Vec8 va{*reinterpret_cast<const uint4*>(base)}, vb{*reinterpret_cast<const uint4*>(base + D / 2)};   // whole-vector loads
+  unpack8(va, a);
+  unpack8(vb, b);
   unpack8(*reinterpret_cast<const Vec8*>(cos_t + static_cast<size_t>(p) * D + vi * 8), c1);
   unpack8(*reinterpret_cast<const Vec8*>(cos_t + static_cast<size_t>(p) * D + D / 2 + vi * 8), c2);
   unpack8(*reinterpret_cast<const Vec8*>(sin_t + static_cast<size_t>(p) * D + vi * 8), s1);

@@ -1,0 +1,629 @@
+// Persistent warp-specialised wgmma GEMM for sm_90a (bf16 x bf16 -> fp32 accumulators in registers -> bf16|fp32).
+//
+//   C[M,N] = op(A) * op(B)      A "K-major":  memory [M, K] row-major        (x, dY)
+//                               A "MN-major": memory [K, M] row-major        (dY^T for wgrad)
+//                               B "K-major":  memory [N, K] row-major        (nn.Linear weight, fwd)
+//                               B "MN-major": memory [K, N] row-major        (weight for dgrad, x for wgrad)
+//
+// This single kernel serves every dense contraction on the DreamLLM hot path (reference call sites:
+// modeling_dreamllm.py:336-338, :395 (q/k/v/o_proj), :237 (gate/up/down_proj), :1452 (lm_head), and their
+// autograd dgrad/wgrad), replacing the cuBLAS calls torch makes for nn.Linear.
+//
+// Structure (one CTA of 384 threads per SM, persistent over a static tile list: CTA c takes tiles c, c + grid, ...):
+//   warpgroup 0     TMA producer (one elected thread): global -> 128B-swizzled smem stages, mbarrier complete_tx
+//   warpgroups 1-2  consumers: each issues wgmma.mma_async (m64 x kBN x k16) for its 64 rows of the 128-row tile, keeps the fp32
+//                   accumulator in registers and runs the epilogue from registers straight to global memory.  The producer keeps
+//                   filling stages for the next tile meanwhile.
+//   setmaxnreg moves registers from the producer warpgroup to the consumers (a 64 x 256 fp32 accumulator is 128 registers a thread).
+#include <stdlib.h>
+
+#include "common.cuh"
+#include "gemm_sm90.h"
+#include "wgmma.cuh"
+
+namespace dllm {
+
+constexpr int BM = 128;  // A rows per CTA (two consumer warpgroups x 64)
+constexpr int BN = 256;  // default N tile (kBN = 128 is instantiated for outputs whose width tiles badly by 256: see pick_bn)
+constexpr int BK = 64;   // 64 bf16 = one 128-byte swizzle line
+constexpr int kGemmThreads = 384;
+
+template <int kBN = BN>
+struct GemmCfg {
+  static constexpr int kABytes = BM * BK * 2;
+  static constexpr int kBBytes = kBN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kBarBytes = 256;
+  // operand stages + barriers <= 227 KB:  kBN 256: 4 stages, kBN 128: 7
+  static constexpr int kStagesFit = (227 * 1024 - kBarBytes - 1024) / kStageBytes;
+  static constexpr int kStages = kStagesFit > 8 ? 8 : kStagesFit;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024 /*align slack*/;
+};
+
+// Fused epilogue:  out = act( bf16(acc + bias[col]) ) (+ residual[row, col])   — rounding points as the reference's
+// unfused bf16 sequence (Linear output rounded, activation rounded, residual add rounded).
+struct GemmEpi {
+  const bf16* bias;      // [N] or nullptr
+  const bf16* residual;  // [M, ldr] or nullptr
+  long ldr;
+  int act;               // 0 none, 1 quick_gelu x*sigmoid(1.702x), 2 gelu (erf), 3 silu
+  const bf16* rowbias;   // [M / rows_per_group, N] or nullptr: per-row-group bias (ResnetBlock2D's time-embedding add)
+  int rows_per_group;
+};
+
+// Implicit-GEMM 3x3 / stride 1 / pad 1 convolution on NHWC activations: A[m, k] = x[n, h + r - 1, w + s - 1, c] with
+// m = (n, h, w), k = (r, s, c).  A 128-row tile is the 4-D TMA box {64 c, Wb, Hb, Nb} (Wb*Hb*Nb = 128) fetched at
+// coordinates (c0, s - 1, h0 + r - 1, n0): out-of-range rows/columns are zero-filled by TMA == the conv's zero padding.
+struct ConvGeom {
+  int cpt;       // Cin / 64: K blocks per filter tap
+  int W, H;      // plane
+  int HW;
+};
+
+__device__ __forceinline__ float epi_act(float x, int act) {
+  if (act == 1) return x / (1.f + expf(-1.702f * x));
+  if (act == 2) return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
+  if (act == 3) return x / (1.f + expf(-x));
+  return x;
+}
+
+__device__ __forceinline__ float2 ld_bf16x2(const bf16* p) {
+  return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+}
+__device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// two adjacent output columns (col, col + 1) of row `row`; `pair` = both in range and the pair is naturally aligned
+template <typename OutT>
+__device__ __forceinline__ void store2(OutT* C, long ldc, int row, int col, int N, bool pair, float x0, float x1) {
+  OutT* p = C + static_cast<size_t>(row) * ldc + col;
+  if constexpr (sizeof(OutT) == 4) {
+    if (pair) { *reinterpret_cast<float2*>(p) = make_float2(x0, x1); return; }
+    p[0] = x0;
+    if (col + 1 < N) p[1] = x1;
+  } else {
+    if (pair) { *reinterpret_cast<uint32_t*>(p) = pack_bf16(x0, x1); return; }
+    p[0] = __float2bfloat16_rn(x0);
+    if (col + 1 < N) p[1] = __float2bfloat16_rn(x1);
+  }
+}
+
+// kEpi: 0 = plain store, 1 = + bias / row-group bias / residual, 2 = 1 + activation, 3 = GEGLU.  Compile-time so that the plain and
+// the bias-only epilogues carry none of the (inlined expf / erff) activation code.
+//
+// ksplit > 1 (split-K, small-M shapes that would leave most SMs idle): a work unit is (output tile, K slice); unit u covers K blocks
+// [ks * kb_per, min(num_kb, (ks + 1) * kb_per)) of tile u / ksplit and stores its fp32 partial at rows ks * Mp + ... of C (the
+// workspace; Mp = M rounded up to whole tiles); splitk_reduce_kernel sums the slices and applies the epilogue.
+template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, OutT* __restrict__ C, long ldc,
+            int M, int N, int K, int group_m, GemmEpi epi, ConvGeom cg, int ksplit) {
+  using Cfg = GemmCfg<kBN>;
+  constexpr int kStages = Cfg::kStages;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + kStages;
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tma_a);
+    tma_prefetch_desc(&tma_b);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  // ---- tile schedule (identical sequence in every role) ----
+  const int num_m_tiles = (M + BM - 1) / BM;
+  const int num_n_tiles = (N + kBN - 1) / kBN;
+  const int num_tiles = num_m_tiles * num_n_tiles * ksplit;       // work units
+  const int num_kb = (K + BK - 1) / BK;
+  const int kb_per = (num_kb + ksplit - 1) / ksplit;
+  const int split_rows = num_m_tiles * BM;                          // Mp: row pitch between K slices in the partial workspace
+  const int tiles_per_group = group_m * num_n_tiles;
+  auto tile_coords = [&](int tile, int& m_blk, int& n_blk) {
+    const int g = tile / tiles_per_group;
+    const int first_m = g * group_m;
+    const int gsize = min(group_m, num_m_tiles - first_m);
+    const int r = tile - g * tiles_per_group;
+    m_blk = first_m + r % gsize;
+    n_blk = r / gsize;
+  };
+
+  if (warp_idx < 4) {
+    // ======================= TMA producer =======================
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && elect_one_sync()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        tile_coords(tile / ksplit, m_blk, n_blk);
+        const int ks = tile % ksplit;
+        const int m0 = m_blk * BM, n0 = n_blk * kBN;
+        for (int kb = ks * kb_per; kb < min(num_kb, (ks + 1) * kb_per); ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1, 1);
+          uint8_t* a_s = smem + stage * Cfg::kStageBytes;
+          uint8_t* b_s = a_s + Cfg::kABytes;
+          const int k0 = kb * BK;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          if constexpr (kConv) {
+            // implicit-conv coordinates of this 128-pixel tile and this K block's filter tap
+            const int tap = kb / cg.cpt;
+            const int cv_c = (kb - tap * cg.cpt) * BK;
+            const int r = tap / 3, sx = tap - 3 * r;
+            const int cv_n = m0 / cg.HW;
+            const int rem = m0 - cv_n * cg.HW;
+            const int h0 = rem / cg.W;
+            const int cv_h = h0 + r - 1;
+            const int cv_w = (rem - h0 * cg.W) + sx - 1;   // non-zero only for planes wider than one 128-pixel tile
+            tma_load_4d(a_s, &tma_a, &full_bar[stage], cv_c, cv_w, cv_h, cv_n);
+          } else if constexpr (!kAMN) {
+            tma_load_2d(a_s, &tma_a, &full_bar[stage], k0, m0);
+          } else {
+#pragma unroll
+            for (int i = 0; i < BM / 64; ++i) tma_load_2d(a_s + i * 8192, &tma_a, &full_bar[stage], m0 + i * 64, k0);
+          }
+          if constexpr (!kBMN) {
+            tma_load_2d(b_s, &tma_b, &full_bar[stage], k0, n0);
+          } else {
+#pragma unroll
+            for (int i = 0; i < kBN / 64; ++i) tma_load_2d(b_s + i * 8192, &tma_b, &full_bar[stage], n0 + i * 64, k0);
+          }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ======================= consumers: wgmma + epilogue =======================
+    setmaxnreg_inc<232>();
+    const int wg = (threadIdx.x >> 7) - 1;   // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+    const int t = threadIdx.x & 127;
+    // accumulator fragment of m64nN: element 4j + 2h + e sits at row 16 * (t / 32) + (t % 32) / 4 + 8h, column 8j + 2 (t % 4) + e
+    const int r_in = 16 * (t >> 5) + ((t & 31) >> 2);
+    const int c_in = 2 * (t & 3);
+    float acc[kBN / 2];
+    // stage-0 descriptors; every other (stage, K step) is that plus a compile-time byte offset (the start-address field counts 16-byte
+    // units and no tile crosses the 256 KB its 14 bits span, so a plain add is exact).  Hoisted, the K block's four wgmma issue back to back.
+    const uint32_t a_s0 = smem_u32(smem) + wg * 8192;   // 64 K-major rows, or MN-major box wg
+    const uint32_t b_s0 = smem_u32(smem) + Cfg::kABytes;
+    const uint64_t adesc0 = kAMN ? make_smem_desc(a_s0, 8192, 1024) : make_smem_desc(a_s0, 16, 1024);
+    const uint64_t bdesc0 = kBMN ? make_smem_desc(b_s0, 8192, 1024) : make_smem_desc(b_s0, 16, 1024);
+    constexpr uint32_t a_step = kAMN ? 2048u : 32u, b_step = kBMN ? 2048u : 32u;   // bytes per K = 16 step
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int m_blk, n_blk;
+      tile_coords(tile / ksplit, m_blk, n_blk);
+      const int ks = tile % ksplit;
+      const int kb0 = ks * kb_per, kb1 = min(num_kb, kb0 + kb_per);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase, 3);
+        const uint64_t soff = static_cast<uint64_t>((stage * Cfg::kStageBytes) >> 4);
+        const uint64_t da = adesc0 + soff, db = bdesc0 + soff;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_ss<kBN, kAMN ? 1 : 0, kBMN ? 1 : 0>(acc, da + ((k * a_step) >> 4), db + ((k * b_step) >> 4), (kb != kb0 || k != 0) ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous K block's MMAs have retired: its stage can be refilled
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue: registers -> global ----
+      const int row_t = m_blk * BM + wg * 64 + r_in;        // + 8h
+      const int col_t = n_blk * kBN + c_in;                 // + 8j
+      const long row_off = (ksplit > 1) ? static_cast<long>(ks) * split_rows : 0;
+      if constexpr (kEpi == 3) {
+        // GEGLU epilogue (diffusers FeedForward: h, gate = proj(x).chunk(2); out = h * gelu(gate)).  The weight rows were permuted at
+        // load time so that every 128-column group of this GEMM's N space is [64 value columns | their 64 gate columns]; a thread
+        // holds value column c and its gate column c + 64 of the same rows and writes column c of the [M, N/2] output — the [M, N]
+        // projection is never written.  Rounding points = the unfused sequence (Linear output to bf16, gelu(gate) to bf16, product to
+        // bf16): bit-identical results.
+        static_assert(kEpi != 3 || sizeof(OutT) == 2, "GEGLU epilogue: bf16 out");
+#pragma unroll
+        for (int pr = 0; pr < kBN / 128; ++pr) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = pr * 16 + jj;
+            const int col = col_t + 8 * j;                  // value column in the permuted N space (gate at + 64)
+            if (col >= N) continue;
+            float2 bv = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+            if (epi.bias != nullptr) { bv = ld_bf16x2(epi.bias + col); bg = ld_bf16x2(epi.bias + col + 64); }
+            const int ocol = (n_blk * kBN >> 1) + pr * 64 + 8 * jj + c_in;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row_t + 8 * h;
+              if (row >= M) continue;
+              float o[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float a = bf16_round(acc[4 * j + 2 * h + e] + (e ? bv.y : bv.x));
+                const float gte = bf16_round(acc[4 * (j + 8) + 2 * h + e] + (e ? bg.y : bg.x));
+                const float gel = bf16_round(0.5f * gte * (1.f + erff(gte * 0.70710678118654752f)));
+                o[e] = a * gel;
+              }
+              store2<OutT>(C, ldc, row, ocol, N >> 1, !(ldc & 1), o[0], o[1]);
+            }
+          }
+        }
+      } else {
+        const bool even_ld = (ldc & 1) == 0;
+#pragma unroll
+        for (int j = 0; j < kBN / 8; ++j) {
+          const int col = col_t + 8 * j;
+          if (col >= N) continue;
+          const bool pair = even_ld && col + 1 < N;
+          float2 bb = make_float2(0.f, 0.f);
+          if (kEpi > 0 && epi.bias != nullptr) bb = ld_bf16x2(epi.bias + col);   // fused epilogues require N % 8 == 0
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row_t + 8 * h;
+            if (row >= M) continue;
+            float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+            if constexpr (kEpi > 0) {
+              x0 += bb.x;
+              x1 += bb.y;
+              if (epi.rowbias != nullptr) {
+                const float2 rb = ld_bf16x2(epi.rowbias + static_cast<size_t>(row / epi.rows_per_group) * N + col);
+                x0 += rb.x;
+                x1 += rb.y;
+              }
+              if constexpr (kEpi == 2) {
+                x0 = bf16_round(x0);
+                x1 = bf16_round(x1);
+                if (epi.act == 1) {
+                  x0 = x0 / (1.f + __expf(-1.702f * x0));
+                  x1 = x1 / (1.f + __expf(-1.702f * x1));
+                } else if (epi.act == 2) {
+                  x0 = 0.5f * x0 * (1.f + erff(x0 * 0.70710678118654752f));
+                  x1 = 0.5f * x1 * (1.f + erff(x1 * 0.70710678118654752f));
+                } else {
+                  x0 = x0 / (1.f + __expf(-x0));
+                  x1 = x1 / (1.f + __expf(-x1));
+                }
+              }
+              if (epi.residual != nullptr) {
+                const float2 rs = ld_bf16x2(epi.residual + static_cast<size_t>(row) * epi.ldr + col);
+                x0 = bf16_round(x0) + rs.x;
+                x1 = bf16_round(x1) + rs.y;
+              }
+            }
+            store2<OutT>(C, ldc, static_cast<int>(row + row_off), col, N, pair, x0, x1);
+          }
+        }
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ host
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static PFN_encodeTiled get_encode_fn() {
+  static PFN_encodeTiled fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return nullptr;
+    fn = reinterpret_cast<PFN_encodeTiled>(p);
+  }
+  return fn;
+}
+
+// 2D row-major tensor [rows, cols] with row stride `ld` elements; box = [box_rows, box_cols]; 128B swizzle.
+int make_tmap_2d(CUtensorMap* map, const void* ptr, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld,
+                 uint32_t box_rows, uint32_t box_cols) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return DLLM_ERR_DRIVER;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * elem_bytes) & 15)) return DLLM_ERR_ALIGN;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstr[1] = {ld * elem_bytes};
+  cuuint32_t box[2] = {box_cols, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = enc(map, dt, 2, const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    fprintf(stderr, "dllm: cuTensorMapEncodeTiled failed (CUresult %d): ptr=%p elem=%d rows=%llu cols=%llu ld=%llu box=[%u x %u]\n",
+            (int)r, ptr, elem_bytes, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, box_cols);
+  return r == CUDA_SUCCESS ? 0 : DLLM_ERR_TMAP;
+}
+
+// SMs left free for a concurrently running collective (NCCL all-reduce overlapped with backward): a persistent GEMM that
+// asks for every SM would have the CTAs that cannot be scheduled wait for the collective kernel to finish and then run
+// their whole static tile list alone.  See dreamllm_b200/ddp.py.
+static int g_reserved_sms = 0;
+void set_reserved_sms(int n) { g_reserved_sms = n < 0 ? 0 : n; }
+int reserved_sms() { return g_reserved_sms; }
+
+int num_sms() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      cudaGetLastError();
+      n = 0;
+      return 132;   // no device visible (build host): plan for an H100 SXM so the workspace queries stay meaningful
+    }
+  }
+  return n;
+}
+
+// N-tile width: 256 (the widest wgmma, half the A re-reads from shared memory per MMA of a 128-wide tile) except for outputs that fit
+// ONE 128-wide tile, where a 256-wide tile would be half padding.
+static inline int pick_bn(int N) { return N <= 128 ? 128 : 256; }
+
+template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN>
+static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
+                          cudaStream_t stream, ConvGeom cg = ConvGeom{1, 1, 1, 1}, int ksplit = 1) {
+  using Cfg = GemmCfg<kBN>;
+  auto kern = gemm_kernel<kAMN, kBMN, OutT, kConv, kEpi, kBN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess)
+      return DLLM_ERR_LAUNCH;
+    attr_set = true;
+  }
+  const int num_tiles = ((M + BM - 1) / BM) * ((N + kBN - 1) / kBN) * ksplit;
+  int avail = num_sms() - g_reserved_sms;
+  if (avail < 1) avail = 1;
+  const int grid = num_tiles < avail ? num_tiles : avail;
+  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, static_cast<OutT*>(C), ldc, M, N, K, 16, epi, cg, ksplit);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+// `bn` must be the value the B tensor map's box was built for (pick_bn(N))
+template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
+                       cudaStream_t stream, ConvGeom cg = ConvGeom{1, 1, 1, 1}, int bn = BN) {
+  if (bn == 128) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 128>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 256>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+}
+
+// ------------------------------------------------------------------------------------------------ split-K (small-M shapes)
+// A [256 x 1280] output over K = 11520 (UNet conv 1280 -> 1280 on the 8x8 plane of 4 samples) is 10 tiles: 10 of 132 SMs busy for
+// 180 K blocks each.  Split-K hands every (tile, K slice) to its own CTA, writes fp32 partials to a caller-provided workspace and lets
+// one small kernel sum them and apply the epilogue with the usual rounding points.
+struct SplitPlan {
+  int bn, ksplit, mp;   // mp = M rounded up to whole tiles
+  size_t ws_bytes;
+};
+static SplitPlan plan_split(int M, int N, int K) {
+  SplitPlan p;
+  p.bn = pick_bn(N);
+  const int mt = (M + BM - 1) / BM, nt = (N + p.bn - 1) / p.bn;
+  const int tiles = mt * nt, num_kb = (K + BK - 1) / BK;
+  int slots = num_sms() - g_reserved_sms;
+  if (slots < 1) slots = 1;
+  int ks = 1;
+  if (tiles * 2 <= slots && num_kb >= 8) {
+    ks = slots / tiles;
+    if (ks > num_kb / 4) ks = num_kb / 4;    // at least 4 K blocks per slice
+    if (ks > 16) ks = 16;
+    if (ks < 2) ks = 1;
+    // no empty slice: the kernel gives every slice ceil(num_kb / ks) K blocks, so the last of e.g. 16 slices of 90 blocks would start
+    // past the end and store an accumulator no MMA ever initialised
+    if (ks > 1) { const int per = (num_kb + ks - 1) / ks; ks = (num_kb + per - 1) / per; }
+  }
+  p.ksplit = ks;
+  p.mp = mt * BM;
+  p.ws_bytes = ks > 1 ? static_cast<size_t>(ks) * p.mp * N * sizeof(float) : 0;
+  return p;
+}
+size_t gemm_splitk_workspace(int M, int N, int K) { return plan_split(M, N, K).ws_bytes; }
+
+// out[m, n] = epilogue( sum_ks ws[ks * mp + m, n] ): bias / row-group bias added in fp32, rounded to bf16, optional activation (rounded),
+// optional residual add (rounded) — the rounding points of gemm_kernel's fused epilogues.  One thread = 8 columns.
+__global__ void splitk_reduce_kernel(const float* __restrict__ ws, bf16* __restrict__ out, long ldc, int M, int N, int mp, int ksplit,
+                                     GemmEpi epi) {
+  const int nvec = N >> 3;
+  const long gid = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (gid >= static_cast<long>(M) * nvec) return;
+  const int v = static_cast<int>(gid % nvec);
+  const int m = static_cast<int>(gid / nvec);
+  float x[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) x[e] = 0.f;
+  for (int ks = 0; ks < ksplit; ++ks) {
+    const float4* p = reinterpret_cast<const float4*>(ws + (static_cast<size_t>(ks) * mp + m) * N + v * 8);
+    const float4 a = p[0], b = p[1];
+    x[0] += a.x; x[1] += a.y; x[2] += a.z; x[3] += a.w; x[4] += b.x; x[5] += b.y; x[6] += b.z; x[7] += b.w;
+  }
+  auto add8 = [&](const bf16* src) {
+    const uint4 q = __ldg(reinterpret_cast<const uint4*>(src));
+    const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { const float2 f = __bfloat1622float2(h2[e]); x[2 * e] += f.x; x[2 * e + 1] += f.y; }
+  };
+  if (epi.bias) add8(epi.bias + v * 8);
+  if (epi.rowbias) add8(epi.rowbias + static_cast<size_t>(m / epi.rows_per_group) * N + v * 8);
+  if (epi.act) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) x[e] = epi_act(__bfloat162float(__float2bfloat16_rn(x[e])), epi.act);
+  }
+  if (epi.residual) {
+    const uint4 q = *reinterpret_cast<const uint4*>(epi.residual + static_cast<size_t>(m) * epi.ldr + v * 8);
+    const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 f = __bfloat1622float2(h2[e]);
+      x[2 * e] = __bfloat162float(__float2bfloat16_rn(x[2 * e])) + f.x;
+      x[2 * e + 1] = __bfloat162float(__float2bfloat16_rn(x[2 * e + 1])) + f.y;
+    }
+  }
+  uint4 o;
+  o.x = pack_bf16(x[0], x[1]); o.y = pack_bf16(x[2], x[3]); o.z = pack_bf16(x[4], x[5]); o.w = pack_bf16(x[6], x[7]);
+  *reinterpret_cast<uint4*>(out + static_cast<size_t>(m) * ldc + v * 8) = o;
+}
+static int launch_splitk_reduce(const void* ws, void* out, long ldc, int M, int N, const SplitPlan& p, const GemmEpi& epi, cudaStream_t st) {
+  const long total = static_cast<long>(M) * (N / 8);
+  splitk_reduce_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>((const float*)ws, (bf16*)out, ldc, M, N, p.mp, p.ksplit, epi);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+
+// bf16-output GEMM (fwd NT or dgrad NN) with the fused-epilogue operands, run as split-K when the shape calls for it and a workspace of
+// gemm_splitk_workspace(M, N, K) bytes is given; otherwise identical to gemm_bf16_ex.
+int gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int b_mn, const void* bias,
+                 const void* residual, long ldr, int act, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const SplitPlan p = plan_split(M, N, K);
+  if (p.ksplit <= 1 || !ws || ws_bytes < p.ws_bytes || (N % 8) || (reinterpret_cast<uintptr_t>(ws) & 15) || (ldc % 8))
+    return gemm_bf16_ex(A, B, C, M, N, K, lda, ldb, ldc, 0, b_mn, 0, -1, bias, residual, ldr, act, stream);
+  if (residual && ((reinterpret_cast<uintptr_t>(residual) & 15) || ((ldr * 2) & 15))) return DLLM_ERR_ALIGN;
+  if (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) return DLLM_ERR_ALIGN;
+  CUtensorMap ta, tb;
+  int rc;
+  if ((rc = make_tmap_2d(&ta, A, 2, M, K, lda, BM, BK))) return rc;
+  if (!b_mn) rc = make_tmap_2d(&tb, B, 2, N, K, ldb, p.bn, BK);
+  else rc = make_tmap_2d(&tb, B, 2, K, N, ldb, BK, 64);
+  if (rc) return rc;
+  GemmEpi none{nullptr, nullptr, 0, 0, nullptr, 1};
+  const ConvGeom nocg{1, 1, 1, 1};
+  if (!b_mn) rc = (p.bn == 128) ? launch_gemm_bn<false, false, float, false, 0, 128>(ta, tb, ws, N, M, N, K, none, stream, nocg, p.ksplit)
+                                : launch_gemm_bn<false, false, float, false, 0, 256>(ta, tb, ws, N, M, N, K, none, stream, nocg, p.ksplit);
+  else rc = (p.bn == 128) ? launch_gemm_bn<false, true, float, false, 0, 128>(ta, tb, ws, N, M, N, K, none, stream, nocg, p.ksplit)
+                          : launch_gemm_bn<false, true, float, false, 0, 256>(ta, tb, ws, N, M, N, K, none, stream, nocg, p.ksplit);
+  if (rc) return rc;
+  GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), ldr, act, nullptr, 1};
+  return launch_splitk_reduce(ws, C, ldc, M, N, p, epi, stream);
+}
+
+int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int a_mn,
+              int b_mn, int out_fp32, int cta_pair, cudaStream_t stream) {
+  return gemm_bf16_ex(A, B, C, M, N, K, lda, ldb, ldc, a_mn, b_mn, out_fp32, cta_pair, nullptr, nullptr, 0, 0, stream);
+}
+
+// cta_pair: kept in the ABI for callers written against two-CTA builds; every tile here is computed by one CTA, so it has no effect.
+int gemm_bf16_ex(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int a_mn,
+                 int b_mn, int out_fp32, int cta_pair, const void* bias, const void* residual, long ldr, int act,
+                 cudaStream_t stream) {
+  (void)cta_pair;
+  if (M <= 0 || N <= 0 || K <= 0 || act < 0 || act > 3) return DLLM_ERR_SHAPE;
+  if ((bias || residual) && (N % 8)) return DLLM_ERR_SHAPE;
+  if (residual && ((reinterpret_cast<uintptr_t>(residual) & 15) || ((ldr * 2) & 15))) return DLLM_ERR_ALIGN;
+  if (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) return DLLM_ERR_ALIGN;
+  if (reinterpret_cast<uintptr_t>(C) & 15) return DLLM_ERR_ALIGN;
+  GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), ldr, act, nullptr, 1};
+  const int bn = pick_bn(N);
+  const ConvGeom nocg{1, 1, 1, 1};
+  CUtensorMap ta, tb;
+  int rc;
+  // A
+  if (!a_mn) rc = make_tmap_2d(&ta, A, 2, M, K, lda, BM, BK);
+  else rc = make_tmap_2d(&ta, A, 2, K, M, lda, BK, 64);
+  if (rc) return rc;
+  // B
+  if (!b_mn) rc = make_tmap_2d(&tb, B, 2, N, K, ldb, bn, BK);
+  else rc = make_tmap_2d(&tb, B, 2, K, N, ldb, BK, 64);
+  if (rc) return rc;
+
+  const int emode = (act != 0) ? 2 : ((bias || residual) ? 1 : 0);
+  if (emode != 0) {
+    // fused epilogues exist for the forward (NT, bf16 out) contraction only
+    if (a_mn || b_mn || out_fp32) return DLLM_ERR_UNSUPPORTED;
+    return emode == 2 ? launch_gemm<false, false, bf16, false, 2>(ta, tb, C, ldc, M, N, K, epi, stream, nocg, bn)
+                      : launch_gemm<false, false, bf16, false, 1>(ta, tb, C, ldc, M, N, K, epi, stream, nocg, bn);
+  }
+#define DLLM_GEMM_CASE(AMN, BMN)                                                                           \
+  if ((a_mn != 0) == AMN && (b_mn != 0) == BMN) {                                                          \
+    return out_fp32 ? launch_gemm<AMN, BMN, float>(ta, tb, C, ldc, M, N, K, epi, stream, nocg, bn)         \
+                    : launch_gemm<AMN, BMN, bf16>(ta, tb, C, ldc, M, N, K, epi, stream, nocg, bn);         \
+  }
+  DLLM_GEMM_CASE(false, false)
+  DLLM_GEMM_CASE(false, true)
+  DLLM_GEMM_CASE(true, true)
+  DLLM_GEMM_CASE(true, false)
+#undef DLLM_GEMM_CASE
+  return DLLM_ERR_SHAPE;
+}
+
+// out[M, N/2] = GEGLU(A @ Wp^T + bias_p): Wp / bias_p are the FeedForward's `proj` weight / bias with rows permuted so that every
+// 128-row group is [64 value rows | the 64 matching gate rows] (dreamllm_b200/unet.py builds them once per frozen UNet).
+int gemm_bf16_geglu(const void* A, const void* Wp, const void* bias_p, void* out, int M, int N, int K, long lda, long ldb, long ldc,
+                    cudaStream_t stream) {
+  if (M <= 0 || N <= 0 || K <= 0 || (N % 128)) return DLLM_ERR_SHAPE;
+  if (bias_p && (reinterpret_cast<uintptr_t>(bias_p) & 15)) return DLLM_ERR_ALIGN;
+  if (reinterpret_cast<uintptr_t>(out) & 15) return DLLM_ERR_ALIGN;
+  GemmEpi epi{static_cast<const bf16*>(bias_p), nullptr, 0, 2, nullptr, 1};
+  CUtensorMap ta, tb;
+  int rc;
+  if ((rc = make_tmap_2d(&ta, A, 2, M, K, lda, BM, BK))) return rc;
+  if ((rc = make_tmap_2d(&tb, Wp, 2, N, K, ldb, BN, BK))) return rc;
+  return launch_gemm_bn<false, false, bf16, false, 3, 256>(ta, tb, out, ldc, M, N, K, epi, stream);
+}
+
+// 4-D NHWC activation map: dims {C, W, H, N}, box {64, Wb, Hb, Nb}, 128B swizzle.
+static int make_tmap_nhwc(CUtensorMap* map, const void* ptr, int Nimg, int H, int W, int C, int Wb, int Hb, int Nb) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return DLLM_ERR_DRIVER;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (C % 8)) return DLLM_ERR_ALIGN;
+  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Nimg};
+  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {64, (cuuint32_t)Wb, (cuuint32_t)Hb, (cuuint32_t)Nb};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), gdim, gstr, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) fprintf(stderr, "dllm: cuTensorMapEncodeTiled(4D) failed (CUresult %d)\n", (int)r);
+  return r == CUDA_SUCCESS ? 0 : DLLM_ERR_TMAP;
+}
+
+size_t conv3x3_splitk_workspace(int Nimg, int H, int W, int Cin, int Cout) {
+  const int M = Nimg * H * W;
+  return plan_split(M, Cout, 9 * Cin).ws_bytes;
+}
+int conv3x3_nhwc(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const void* bias,
+                 const void* rowbias, const void* residual, cudaStream_t stream) {
+  return conv3x3_nhwc_ws(x, w, y, Nimg, H, W, Cin, Cout, bias, rowbias, residual, nullptr, 0, stream);
+}
+// y[n,h,w,:] = conv3x3(x, w) + bias + rowbias[n] (+ residual);  x NHWC [Nimg,H,W,Cin], w [Cout, 3,3,Cin] (K-major), y NHWC.
+// With a workspace of conv3x3_splitk_workspace() bytes small planes run split-K (see plan_split).
+int conv3x3_nhwc_ws(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const void* bias,
+                    const void* rowbias, const void* residual, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  if (Nimg <= 0 || Cin % 64 || Cout % 8) return DLLM_ERR_SHAPE;
+  if (W > 128 ? (W % 128) : (128 % W)) return DLLM_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(y) & 15) return DLLM_ERR_ALIGN;
+  const int HW = H * W;
+  int Wb = W > 128 ? 128 : W, Hb = W > 128 ? 1 : 128 / W, Nb = 1;
+  if (Hb > H) {  // small planes: the 128-pixel tile spans several whole images
+    if (Hb % H) return DLLM_ERR_SHAPE;
+    Nb = Hb / H;
+    Hb = H;
+  } else if (H % Hb) {
+    return DLLM_ERR_SHAPE;
+  }
+  const int M = Nimg * HW, K = 9 * Cin;
+  const int bn = pick_bn(Cout);
+  CUtensorMap ta, tb;
+  int rc;
+  if ((rc = make_tmap_nhwc(&ta, x, Nimg, H, W, Cin, Wb, Hb, Nb))) return rc;
+  if ((rc = make_tmap_2d(&tb, w, 2, Cout, K, K, bn, BK))) return rc;
+  GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), Cout, 0, static_cast<const bf16*>(rowbias), HW};
+  ConvGeom cg{Cin / 64, W, H, HW};
+  const SplitPlan sp = plan_split(M, Cout, K);
+  if (sp.ksplit > 1 && ws && ws_bytes >= sp.ws_bytes && !(reinterpret_cast<uintptr_t>(ws) & 15)) {
+    GemmEpi none{nullptr, nullptr, 0, 0, nullptr, 1};
+    rc = (bn == 128) ? launch_gemm_bn<false, false, float, true, 0, 128>(ta, tb, ws, Cout, M, Cout, K, none, stream, cg, sp.ksplit)
+                     : launch_gemm_bn<false, false, float, true, 0, 256>(ta, tb, ws, Cout, M, Cout, K, none, stream, cg, sp.ksplit);
+    if (rc) return rc;
+    return launch_splitk_reduce(ws, y, Cout, M, Cout, sp, epi, stream);
+  }
+  const bool any_epi = bias || rowbias || residual;
+  return any_epi ? launch_gemm<false, false, bf16, true, 1>(ta, tb, y, Cout, M, Cout, K, epi, stream, cg, bn)
+                 : launch_gemm<false, false, bf16, true, 0>(ta, tb, y, Cout, M, Cout, K, epi, stream, cg, bn);
+}
+
+}  // namespace dllm

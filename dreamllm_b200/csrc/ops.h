@@ -1,4 +1,4 @@
-// Internal C++ declarations of the non-GEMM ops (definitions: elementwise.cu, attn_sm100.cu).
+// Internal C++ declarations of the non-GEMM ops (definitions: elementwise.cu, attn_sm90.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -60,7 +60,6 @@ int attn_bwd_ex(const void* dout, const void* q, const void* k, const void* v, c
                 int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, cudaStream_t s);
 int groupnorm_bwd_nhwc(const void* dy, const void* x, const void* w, const void* b, const float* stats, const void* dres, void* dx,
                        void* workspace, size_t ws_bytes, int N, int HW, int C, int G, int silu, cudaStream_t s);
-void attn_item_order(int w, int ntiles, int n_hb, int grid, int descending, int* tile, int* hb, int* win_heads_out);
 int groupnorm_stats(const void* x, float* stats, void* workspace, size_t ws_bytes, int N, int HW, int C, int G, float eps, cudaStream_t s);
 int groupnorm_apply(const void* x, const void* w, const void* b, const float* stats, void* y, int N, int HW, int C, int G, int silu,
                     cudaStream_t s);

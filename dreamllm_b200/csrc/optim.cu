@@ -1,11 +1,11 @@
-// Sharded AdamW step + gradient sum-of-squares for the data-parallel optimizer (SURVEY.md §8f row 4; sm_100a).
+// Sharded AdamW step + gradient sum-of-squares for the data-parallel optimizer (SURVEY.md §8f row 4; sm_90a).
 //
 // Replaces, for one rank's shard of a flat gradient bucket, what the reference gets from HF Trainer:
 //   `optim="adamw_torch"` (projects/dreamllm/configs/stage1/base.py:85, stage2/base.py:95) on a model loaded in bf16
 //   (projects/dreamllm/train.py:68-70, :138) under FSDP `shard_grad_op` (stage2/base.py:91-94), with
 //   `clip_grad_norm_(max_grad_norm)` before the step (omni/train/trainer.py:800-807).
 //
-// Both kernels are HBM-bound streaming passes (no reuse): 128-bit vector accesses, grid-stride over 148 x 8 CTAs.
+// Both kernels are HBM-bound streaming passes (no reuse): 128-bit vector accesses, grid-stride over 132 x 8 CTAs (one H100 SXM).
 //   adamw_kernel<false>: fp32 master / m / v shard, bf16 grad in, bf16 param out : 14 B read + 14 B written per element
 //   adamw_kernel<true> : bf16 param / m / v (the reference's arithmetic: every ATen op of torch.optim.AdamW's
 //                        single-tensor path rounds its result to bf16)          :  8 B read +  6 B written per element
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(256) adamw_kernel(const BVec8* __restrict__ gr
   }
 }
 
-constexpr int kSumsqBlocks = 148 * 4;
+constexpr int kSumsqBlocks = 132 * 4;   // 4 CTAs per H100 SM
 
 __global__ void __launch_bounds__(256) sumsq_partial_kernel(const BVec8* __restrict__ x, long nvec, float* __restrict__ partials) {
   __shared__ float red[8];
@@ -185,7 +185,7 @@ int adamw_step(const void* grad, void* master, void* mom, void* var, void* param
   a.neg_step = static_cast<float>(-(lr / bc1));
   a.max_norm = static_cast<float>(max_norm);
   const long nvec = n >> 3;
-  const int blocks = static_cast<int>(std::min<long>((nvec + 255) / 256, 148L * 8));
+  const int blocks = static_cast<int>(std::min<long>((nvec + 255) / 256, 132L * 8));
   if (bf16_state)
     adamw_kernel<true><<<blocks, 256, 0, s>>>(reinterpret_cast<const BVec8*>(grad), nullptr, mom, var, reinterpret_cast<BVec8*>(param),
                                               nvec, a, sumsq);

@@ -1,9 +1,9 @@
-// HBM-bound kernels of the SD-2.1 UNet denoising step (sm_100a), NHWC bf16 activations.
+// HBM-bound kernels of the SD-2.1 UNet denoising step (sm_90a), NHWC bf16 activations.
 // Reference call sites: StableDiffusionHead.pipeline, modeling_plugins.py:809-833 (unet(...) -> CFG combine ->
 // scheduler.step), whose arithmetic is diffusers 0.24 (ResnetBlock2D GroupNorm+SiLU, GEGLU, Upsample2D, Downsample2D,
 // Timesteps, DDIM/DDPM step) — restated in oracle/unet_oracle.py.
 #include "common.cuh"
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 #include "ops.h"
 
 namespace dllm {
@@ -286,11 +286,11 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(const bf16* __r
 }
 
 // pixel rows per partial-sum CTA: 64 for the big UNet planes, more for the VAE's 512x512 planes so that the finalize pass never walks
-// more than 128 partials, fewer for small planes so that the grid still covers the 148 SMs
+// more than 128 partials, fewer for small planes so that the grid still covers every SM
 static inline int gn_rows(int HW, int N) {
   int rows = 256;                                  // enough rows per CTA to amortise the per-CTA prologue / reduction epilogue ...
   while ((HW + rows - 1) / rows > 128) rows *= 2;
-  while (rows > 8 && static_cast<long>(N) * ((HW + rows - 1) / rows) < 4 * 148 && (HW + rows / 2 - 1) / (rows / 2) <= 128) rows /= 2;   // ... but >= 4 CTAs / SM
+  while (rows > 8 && static_cast<long>(N) * ((HW + rows - 1) / rows) < 4 * num_sms() && (HW + rows / 2 - 1) / (rows / 2) <= 128) rows /= 2;   // ... but >= 4 CTAs / SM
   return rows;
 }
 size_t groupnorm_workspace(int N, int HW, int G) {
@@ -316,7 +316,7 @@ static void gn_launch_apply(const bf16* x, const bf16* w, const bf16* b, const f
                             cudaStream_t s) {
   const GnMap m = gn_map(C);
   int rows = 128;
-  while (rows > m.RL && static_cast<long>(N) * ((HW + rows - 1) / rows) < 4 * 148) rows /= 2;
+  while (rows > m.RL && static_cast<long>(N) * ((HW + rows - 1) / rows) < 4 * num_sms()) rows /= 2;
   gn_apply_kernel<false><<<dim3((HW + rows - 1) / rows, N), m.threads, 0, s>>>(x, nullptr, w, b, stats, nullptr, nullptr, y, HW, C, G, rows,
                                                                                 m.RL, silu);
 }
@@ -544,7 +544,7 @@ int conv_out_nhwc_to_nchw(const void* x, const void* w, const void* bias, float*
 // ---- conv_in / conv_out on the tensor cores (round 2).  The direct kernels above cost 1.36 ms (conv_in, 4 -> 320 @ 64x64 x 32) and
 // 0.68 ms (conv_out) of a 42 ms UNet step, and 0.95 ms per VAE conv_in at 512x512 (profiles/r02d_unet_launch_list_summary.md):
 //   conv_in  = im2col of the tiny-Cin fp32 NCHW input into bf16 rows [M, 64] (k = (c*3 + r)*3 + s, zero padded to one 64-wide K block)
-//              + the tcgen05 GEMM with the bias epilogue against the [Cout, 64] weight matrix          (dllm_im2col_in + dllm_gemm_bf16_ex)
+//              + the wgmma GEMM with the bias epilogue against the [Cout, 64] weight matrix          (dllm_im2col_in + dllm_gemm_bf16_ex)
 //   conv_out = the implicit-GEMM conv3x3 with Cout zero-padded to 8 + a channel-slicing NHWC bf16 -> NCHW fp32 pass
 //                                                                                                    (dllm_conv3x3_nhwc + dllm_nhwc_to_nchw_f32)
 __global__ void im2col_in_kernel(const float* __restrict__ x, bf16* __restrict__ cols, long total_vec, int Bsrc, int Cin, int H, int W) {
@@ -680,7 +680,7 @@ int groupnorm_bwd_nhwc(const void* dy, const void* x, const void* w, const void*
       (const bf16*)x, (const bf16*)dy, (const bf16*)w, (const bf16*)b, stats, partial, HW, C, G, rows, m.RL, silu);
   gn_finalize_kernel<<<(N * G * 32 + 255) / 256, 256, 0, s>>>(partial, sums, nchunks, G, static_cast<float>(HW) * (C / G), -1.f, N * G);
   int arows = 128;
-  while (arows > m.RL && static_cast<long>(N) * ((HW + arows - 1) / arows) < 4 * 148) arows /= 2;
+  while (arows > m.RL && static_cast<long>(N) * ((HW + arows - 1) / arows) < 4 * num_sms()) arows /= 2;
   gn_apply_kernel<true><<<dim3((HW + arows - 1) / arows, N), m.threads, 0, s>>>((const bf16*)x, (const bf16*)dy, (const bf16*)w,
                                                                                 (const bf16*)b, stats, sums, (const bf16*)dres, (bf16*)dx,
                                                                                 HW, C, G, arows, m.RL, silu);

@@ -26,12 +26,12 @@ import torch
 import torch.distributed as dist
 
 NCCL_CTAS = int(_os.environ.get("DLLM_NCCL_CTAS", "0"))        # SM budget handed to the overlapped all-reduce (0 = leave NCCL alone)
-RESERVED_SMS = int(_os.environ.get("DLLM_RESERVED_SMS", "0"))  # CTA pairs kept out of the persistent GEMM grids while grads are in flight
+RESERVED_SMS = int(_os.environ.get("DLLM_RESERVED_SMS", "0"))  # SMs kept out of the persistent GEMM grids while grads are in flight
 
 
 def configure_nccl_env():
-    """Optional knobs (off by default — measured on 2 x B200, ms/step: NCCL default + dynamic GEMM scheduler is best;
-    capping NCCL to 2 CTAs exposes the all-reduce: 799 ms; reserving SMs for it: 704 ms; see profiles/r01_ddp_n2_variants.md)."""
+    """Optional knobs, off by default: NCCL_MAX_CTAS caps the all-reduce's CTAs, reserved SMs keep the persistent GEMM grids off SMs the
+    overlapped all-reduce occupies.  Whether either helps on a given multi-GPU H100 box has to be measured there."""
     import os
     if NCCL_CTAS > 0:
         os.environ.setdefault("NCCL_MAX_CTAS", str(NCCL_CTAS))

@@ -1,4 +1,4 @@
-"""B200-native mirror of the reference's `omni/models/dreamllm/modeling_dreamllm.py` decoder stack.
+"""H100-native mirror of the reference's `omni/models/dreamllm/modeling_dreamllm.py` decoder stack.
 
 Same class names, constructor / forward signatures, parameter names and state-dict keys as the reference
 (SURVEY.md §8b) so the classes drop into `omni.models.dreamllm`; all arithmetic runs in libdreamllm_sm100.so.

@@ -1,4 +1,4 @@
-"""B200-native mirror of `omni/models/dreamllm/modeling_plugins.py` (plugin ABCs :32-112, DreamEmbedding :116-181,
+"""H100-native mirror of `omni/models/dreamllm/modeling_plugins.py` (plugin ABCs :32-112, DreamEmbedding :116-181,
 CLIPVisionEmbedding :184-331) plus the index plumbing of the embedding splice / conditioning gather
 (modeling_dreamllm.py:1082-1141, :1401-1418).
 

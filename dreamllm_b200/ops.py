@@ -71,7 +71,7 @@ ACT_NONE, ACT_QUICK_GELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
 def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, out: torch.Tensor | None = None,
          out_dtype=BF16, cta_pair: int = -1, bias: torch.Tensor | None = None, residual: torch.Tensor | None = None,
          act: int = 0) -> torch.Tensor:
-    """C[M,N] = op(A) @ op(B) on tcgen05.
+    """C[M,N] = op(A) @ op(B) on wgmma.
 
     a_mn=False: a is [M,K];  a_mn=True: a is [K,M] (uses a^T)
     b_mn=False: b is [N,K] (nn.Linear weight layout, C = A @ B^T);  b_mn=True: b is [K,N] (C = A @ B)
@@ -639,7 +639,7 @@ def _cached_weight(key, w, build):
 
 
 def conv_in(latents_nchw_f32, weight, bias, batch_out):
-    """Conv2d(Cin <= 7, Cout, 3, pad 1) on fp32 NCHW latents / images -> NHWC bf16, as im2col ([M, 64] bf16) + tcgen05 GEMM with the bias
+    """Conv2d(Cin <= 7, Cout, 3, pad 1) on fp32 NCHW latents / images -> NHWC bf16, as im2col ([M, 64] bf16) + wgmma GEMM with the bias
     epilogue (the direct kernel `dllm_conv_in` cost 1.4 ms per UNet step and 0.95 ms per VAE encode)."""
     Bs, Cin, H, W = latents_nchw_f32.shape
     Cout = weight.shape[0]

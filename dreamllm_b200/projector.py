@@ -1,8 +1,8 @@
-"""B200-native mirror of `omni/models/projector` (builder.py:10-22, mlp_projector.py:11-50, base_projector.py:8-36).
+"""H100-native mirror of `omni/models/projector` (builder.py:10-22, mlp_projector.py:11-50, base_projector.py:8-36).
 
 Same API: `build_projector(projector_cfg, in_hidden_size, out_hidden_size, bias)` returns a module with a `.projector`
 submodule (state-dict key `projector.weight` / `projector.{0,2,..}.weight`), whose `forward(features | list)` returns a
-**list** of tensors (callers take `[-1]`, modeling_plugins.py:325, :546).  Arithmetic: tcgen05 GEMM with fused bias /
+**list** of tensors (callers take `[-1]`, modeling_plugins.py:325, :546).  Arithmetic: wgmma GEMM with fused bias /
 GELU epilogue; backward = dgrad + wgrad GEMMs + bias column-sum.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""B200-native SD-2.1 `UNet2DConditionModel` (forward / denoising) and the CUDA-graph sampler loop.
+"""H100-native SD-2.1 `UNet2DConditionModel` (forward / denoising) and the CUDA-graph sampler loop.
 
 Reference call sites: `StableDiffusionHead.pipeline`, modeling_plugins.py:672-850 — per step
 `cat([latents]*2) -> scale_model_input -> unet(latent_model_input, t, encoder_hidden_states=prompt_embeds).sample -> chunk ->
@@ -6,10 +6,10 @@ eps_u + g (eps_c - eps_u) -> scheduler.step` (:809-833).  The UNet / scheduler a
 module tree and parameter names below are diffusers' (state-dict compatible: 686 keys, 865 910 724 parameters), the restated
 oracle is oracle/unet_oracle.py (SURVEY.md Appendix A.1 / A.2).
 
-B200 design (SURVEY §8 rows U1-U6, a15, a16):
-  * activations NHWC bf16; every 3x3 conv is an implicit GEMM on tcgen05 (4-D TMA im2col with zero-fill padding), 1x1 convs and all
+Design (SURVEY §8 rows U1-U6, a15, a16):
+  * activations NHWC bf16; every 3x3 conv is an implicit GEMM on wgmma (4-D TMA im2col with zero-fill padding), 1x1 convs and all
     Linear layers are the same GEMM kernel with fused bias / time-embedding row-bias / residual epilogues;
-  * self-attention (seq 4096/1024/256/64, d = 64) and cross-attention on the dream-query conditioning (kv len 64 / 77) use the tcgen05
+  * self-attention (seq 4096/1024/256/64, d = 64) and cross-attention on the dream-query conditioning (kv len 64 / 77) use the wgmma
     flash-attention kernel; the cross-attention K/V projections are timestep-invariant and computed ONCE per prompt, outside the loop;
   * GroupNorm(+SiLU), LayerNorm, GEGLU, upsample, concat are single-pass HBM-bound kernels;
   * the step (time embedding -> UNet -> fused CFG + DDIM/DDPM update) is captured once in a CUDA graph and replayed; the timestep and

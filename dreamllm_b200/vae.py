@@ -1,4 +1,4 @@
-"""B200-native SD `AutoencoderKL` ENCODER (forward only; frozen tower: freeze_vae=True) for the diffusion-loss path.
+"""H100-native SD `AutoencoderKL` ENCODER (forward only; frozen tower: freeze_vae=True) for the diffusion-loss path.
 
 Reference call site: `latents = self.vae.encode(images).latent_dist.sample() * scaling_factor`, modeling_plugins.py:511-512
 (arithmetic: diffusers 0.24 AutoencoderKL, SURVEY.md Appendix A.3 / §8(f) row 1; oracle: oracle/vae_oracle.py, diffusers key names:

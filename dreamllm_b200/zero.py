@@ -6,7 +6,7 @@ gradient clipping at `max_grad_norm` (omni/train/trainer.py:800-807) and a cosin
 (stage1/base.py:76-77).  `shard_grad_op` = parameters stay whole through forward and backward, gradients are reduce-scattered,
 each rank owns 1/N of the optimizer state — ZeRO stage 2.
 
-B200 design (one process per GPU, torch.distributed only as transport):
+Design (one process per GPU, torch.distributed only as transport):
 
 * parameters are re-seated as views of flat bf16 buckets (forward order inside a bucket, so the fused q|k|v and gate|up row blocks of
   `modeling_dreamllm._fuse_rows` stay adjacent); gradients land in a mirror-image flat bucket;

@@ -1,4 +1,4 @@
-/* libdreamllm_sm100.so — C ABI of the B200-native DreamLLM hot path.
+/* libdreamllm_sm100.so — C ABI of the H100-native (sm_90a) DreamLLM hot path.
  *
  * The reference (RunpeiDong/DreamLLM) is pure Python and has no FFI of its own (SURVEY.md §8b); these entry points
  * are what a ctypes / cffi binding inside `omni/models/dreamllm` calls in place of the torch ops the reference
@@ -31,10 +31,10 @@ const char* dllm_error_string(int code);
 int dllm_set_reserved_sms(int n);
 int dllm_get_reserved_sms(void);
 
-/* Dense contraction on tcgen05 tensor cores: C[M,N] = op(A) * op(B), fp32 accumulate in TMEM.
+/* Dense contraction on wgmma tensor cores: C[M,N] = op(A) * op(B), fp32 accumulate in registers.
  *   a_mn = 0: A is [M,K] row-major; a_mn = 1: A is stored [K,M] row-major (i.e. A^T, used for wgrad)
  *   b_mn = 0: B is [N,K] row-major (an nn.Linear weight); b_mn = 1: B is stored [K,N] row-major
- *   out_fp32: C dtype (0 = bf16, 1 = fp32).  cta_pair: -1 auto, 0 = one CTA per tile, 1 = cta_group::2 pairs.
+ *   out_fp32: C dtype (0 = bf16, 1 = fp32).  cta_pair: accepted for compatibility, no effect (one CTA per tile).
  * Replaces F.linear / nn.Linear and their autograd dgrad/wgrad:
  *   modeling_dreamllm.py:336-338, :395 (q/k/v/o_proj), :237 (gate/up/down_proj), :1452 (lm_head),
  *   omni/models/projector/mlp_projector.py:11-50 (projectors). */
@@ -74,7 +74,7 @@ int dllm_embedding_fwd(const long long* ids, const void* weight, void* out, int 
 int dllm_embedding_bwd(const long long* sorted_ids, const long long* order, const void* dy, void* dweight, int T,
                        int H, int accumulate, void* stream);
 
-/* Causal / full flash attention on tcgen05 (replaces flash_attn_func / flash_attn_varlen_func,
+/* Causal / full flash attention on wgmma tensor cores (replaces flash_attn_func / flash_attn_varlen_func,
  * modeling_dreamllm.py:500-551, and the eager path :357-379).
  * q,k,v: [B, S, nh, d] views with row stride ld_qkv (elements) between consecutive tokens — the fused qkv GEMM
  * output is consumed directly, no transposes.  out: [B, S, nh*d] (ld_o).  lse: [B, nh, S] fp32.
@@ -122,7 +122,7 @@ int dllm_attn_fwd_cache(const void* q, const void* k, const void* v, void* out, 
 int dllm_attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, float* lse, const void* kv_mask, int mask_ld, int B,
                              int Sq, int Skv, int kv_rows, int nh, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale,
                              void* stream);
-/* ResnetBlock2D / Upsample2D conv: implicit-GEMM 3x3 stride-1 pad-1 on tcgen05 (4-D TMA im2col, zero-fill padding).
+/* ResnetBlock2D / Upsample2D conv: implicit-GEMM 3x3 stride-1 pad-1 on wgmma tensor cores (4-D TMA im2col, zero-fill padding).
  * y = conv(x, w) + bias[c] + rowbias[n, c] (+ residual);  w is [Cout, 3, 3, Cin]. */
 int dllm_conv3x3_nhwc(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, const void* bias,
                       const void* rowbias, const void* residual, void* stream);
@@ -172,11 +172,6 @@ int dllm_sampler_step(const float* eps, float* latents, const float* noise, cons
 int dllm_attn_bwd_ex(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
                      void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int Sq, int Skv, int nh,
                      int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, void* stream);
-/* Host-only: the order in which the persistent attention kernels (flash attention replacing flash_attn_func / flash_attn_varlen_func,
- * modeling_dreamllm.py:532-551) hand out their (tile, head x batch) work items — item w of a launch with `grid` resident CTAs.  Windows of
- * win_heads = ceil(2 * grid / ntiles) consecutive (head, batch) pairs; inside a window heaviest tiles first (descending != 0: highest
- * tile index first — forward / dQ under a causal mask; 0: lowest first — dK/dV).  For tests and tooling; no device work. */
-void dllm_attn_item_order(int w, int ntiles, int n_hb, int grid, int descending, int* tile, int* hb, int* win_heads);
 int dllm_groupnorm_stats(const void* x, float* stats, void* workspace, size_t ws_bytes, int N, int HW, int C, int G, float eps, void* stream);
 int dllm_groupnorm_apply(const void* x, const void* w, const void* b, const float* stats, void* y, int N, int HW, int C, int G, int silu,
                          void* stream);

@@ -29,7 +29,7 @@ CASES = [
     # BASELINE.json configs[0] itself: Vicuna-7B layer, hidden 4096, 32 heads, seq 512, bs 1 (y / dx stored strided to keep the file small)
     ("c1", 4096, 11008, 32, 1, 512, 14, 0),
 ]
-STRIDED = {"c1": (4, 8)}        # name -> (row step, column step) of the stored y / dx
+STRIDED = {"c1": (4, 8), "mid": (2, 1)}        # name -> (row step, column step) of the stored y / dx (files stay under 1 MB)
 
 
 def make_inputs(hidden, bsz, seq, seed):

@@ -1,4 +1,4 @@
-"""CPU-side checks of the C-ABI boundary: the library builds for sm_100a, loads without a GPU, exports every
+"""CPU-side checks of the C-ABI boundary: the library builds for sm_90a, loads without a GPU, exports every
 symbol include/dreamllm_sm100.h declares, and the product path fails loudly (no CPU fallback)."""
 import os
 import re
@@ -29,54 +29,47 @@ def test_library_exports_every_declared_symbol():
     assert L.dllm_attn_bwd_workspace_bytes(2, 100, 4, 128) == 2 * 128 * 4 * 2 * 4
 
 
-def test_sass_contains_tcgen05_and_tma():
-    """The shipped cubin is Blackwell-native: tcgen05.mma (UTC*MMA), TMEM loads (LDTM), TMA (UTMALDG/UTMASTG)."""
+def test_sass_contains_wgmma_and_tma():
+    """The shipped cubin is Hopper-native: warpgroup MMA (HGMMA) fed by TMA loads (UTMALDG), every kernel built for sm_90a."""
     import subprocess
     from dreamllm_b200 import _lib
     _lib.build()
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "LDTM", "UTMALDG", "UTMASTG"):
+    for mnem in ("HGMMA", "UTMALDG"):
         assert mnem in sass, mnem
     assert "HMMA.16816" not in sass      # no legacy mma.sync path
+    archs = set(re.findall(r"arch = (sm_\w+)", sass))
+    assert archs == {"sm_90a"}, archs
 
 
 def test_tile_gemm_mma_instructions_are_issued_back_to_back():
-    """Regression guard for the round-2 issue-path fix (profiles/r02j_attn_fwd_timeline.md): inside a tile-GEMM the UTCHMMAs must follow each
-    other directly.  With the issuer chosen by `lane == 0` ptxas wrapped every UTCHMMA in an ELECT / BRA.U.ANY loop and rebuilt the
-    operand descriptors per K step: 13 (attention) to 21 (GEMM) dependent scalar instructions ~ 100 clk between two MMAs that occupy the
-    tensor pipe for 32-128 clk.  Checked per kernel: most consecutive-UTCHMMA gaps are <= 4 instructions and none of the *typical* ones
-    (the median) exceeds 3."""
-    import re
+    """Regression guard for the issue path of the warpgroup MMAs.  Inside one wgmma commit group (the HGMMAs up to the one that carries
+    `gsb0`) no WARPGROUP.DEPBAR, barrier or call may separate two HGMMAs: a function call reachable from the wgmma region (printf in the
+    bounded mbarrier wait) once made ptxas serialise every wgmma (C7510, a DEPBAR after each HGMMA).  And the HGMMAs of a group follow
+    each other closely (median gap <= 8 instructions): rebuilding the smem descriptors per K step put 11-13 instructions between them."""
     import statistics
     import subprocess
     from dreamllm_b200 import _lib
     _lib.build()
     bdir = os.path.join(os.path.dirname(_lib.LIB_PATH), "build")
     checked = 0
-    for obj in ("gemm_sm100.o", "attn_sm100.o"):
+    for obj in ("gemm_sm90.o", "attn_sm90.o"):
         sass = subprocess.run(["cuobjdump", "-sass", os.path.join(bdir, obj)], capture_output=True, text=True).stdout
-        cur, idx, n = None, [], 0
-        funcs = {}
-        for line in sass.splitlines():
-            m = re.search(r"Function : (\S+)", line)
-            if m:
-                cur, n = m.group(1), 0
-                funcs[cur] = []
-                continue
-            if cur and re.match(r"\s+/\*[0-9a-f]{4}\*/", line):
-                n += 1
-                if "UTCHMMA" in line:
-                    funcs[cur].append(n)
-        for name, pos in funcs.items():
+        for body in re.split(r"Function : ", sass)[1:]:
+            name = body.split("\n", 1)[0]
+            ins = [ln for ln in body.splitlines() if re.match(r"\s+/\*[0-9a-f]{4}\*/", ln)]
+            pos = [i for i, ln in enumerate(ins) if "HGMMA" in ln]
             if len(pos) < 4:
                 continue
-            if "attn_" in name and "persist" not in name and "_ts_" not in name and "attn_fwd_kernel" not in name:
-                continue                                   # round-1 data-path kernels kept only for DLLM_ATTN_LEGACY A/B runs
-            gaps = [b - a for a, b in zip(pos, pos[1:])]
-            assert statistics.median(gaps) <= 3, (name[:80], gaps)
-            assert sum(g <= 4 for g in gaps) >= 0.6 * len(gaps), (name[:80], gaps)
+            gaps = []
+            for a, b in zip(pos, pos[1:]):
+                if "gsb0" in ins[a]:                       # end of a commit group: waits may follow
+                    continue
+                assert not any(m in ln for ln in ins[a + 1:b] for m in ("DEPBAR", "BAR.SYNC", "CALL")), (name[:80], ins[a + 1:b])
+                gaps.append(b - a)
+            assert gaps and statistics.median(gaps) <= 8, (name[:80], gaps)
             checked += 1
-    assert checked >= 20, checked
+    assert checked >= 30, checked
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
@@ -110,23 +103,20 @@ def test_host_only_entry_points_answer_without_a_gpu():
     assert L.dllm_attn_bwd_workspace_bytes(8, 2048, 32, 128) >= 8 * 32 * 2048 * 4        # at least the fp32 row term D = rowsum(dO * O)
     assert L.dllm_attn_bwd_workspace_bytes(8, 2048, 32, 128) > L.dllm_attn_bwd_workspace_bytes(1, 512, 32, 128)
     assert L.dllm_groupnorm_workspace_bytes(16, 64 * 64, 32) > 0
-    assert L.dllm_sumsq_workspace_bytes() == 148 * 4 * 4
+    assert L.dllm_sumsq_workspace_bytes() == 132 * 4 * 4
     assert L.dllm_get_reserved_sms() == 0
 
 
 def test_split_k_plan_never_has_an_empty_slice():
-    """`dllm_gemm_splitk_workspace_bytes` / `dllm_conv3x3_splitk_workspace_bytes` are host code (148 SMs assumed without a device): the
+    """`dllm_gemm_splitk_workspace_bytes` / `dllm_conv3x3_splitk_workspace_bytes` are host code (132 SMs assumed without a device): the
     slice count they imply must divide the K blocks without an empty last slice.  The kernel gives every slice ceil(num_kb / ks) blocks, so
     ks = 16 over 90 blocks made slice 15 start past the end and store an accumulator no MMA had initialised (round 2, caught by the conv
     parity test on the GPU); small outputs must be split, full waves must not."""
     from dreamllm_b200 import _lib
     L = _lib.lib()
-    if os.environ.get("DLLM_GEMM_NO_SPLITK") == "1":
-        pytest.skip("split-K disabled by environment")
 
     def check(ws, M, N, K):
-        tile_m = 256 if M > 128 else 128
-        mp = (M + tile_m - 1) // tile_m * tile_m
+        mp = (M + 127) // 128 * 128
         assert ws % (mp * N * 4) == 0, (M, N, K, ws)
         ks = ws // (mp * N * 4)
         num_kb = (K + 63) // 64

@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (fwd + two-kernel bwd) vs the CPU oracle's eager softmax(QK^T/sqrt(d)+mask)V
+"""wgmma flash attention (fwd + two-kernel bwd) vs the CPU oracle's eager softmax(QK^T/sqrt(d)+mask)V
 (oracle.decoder_oracle.attention_eager's core, reference modeling_dreamllm.py:357-379) on seeded inputs."""
 import math
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM parity (through the C ABI) vs an fp32 torch reference of the same contraction."""
+"""wgmma GEMM parity (through the C ABI) vs an fp32 torch reference of the same contraction."""
 import pytest
 import torch
 
@@ -9,7 +9,7 @@ SHAPES = [
     (128, 256, 64),
     (256, 256, 128),
     (512, 4096, 4096),      # C1 q/k/v/o projection
-    (384, 768, 320),        # tails in M (2-CTA), N; K not a multiple of 64
+    (384, 768, 320),        # tails in M, N; K not a multiple of 64
     (200, 264, 72),         # ragged everything (multiples of 8 only)
     (1024, 1408, 512),
     # widths served by the 128-wide N tile (pick_bn: less padded MMA work than 256): VAE C = 128, UNet C = 320 / 640

@@ -11,7 +11,7 @@ from dreamllm_b200.configuration_dreamllm import ConfigAndInitKwargs, DreamLLMCo
 from dreamllm_b200.modeling_dreamllm import DreamLLMForCausalMLM, KVCache
 from dreamllm_b200.modeling_plugins import DreamEmbedding
 
-REF_CFG = "/root/reference/omni/models/dreamllm/configuration_dreamllm.py"
+REF_CFG = os.path.join(os.path.dirname(__file__), "golden", "reference_config.json")
 TINY = dict(vocab_size=96, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2)
 
 
@@ -28,31 +28,22 @@ class Tok:
         return [table[x] for x in t] if isinstance(t, list) else table[t]
 
 
-@pytest.mark.skipif(not os.path.isfile(REF_CFG), reason="reference checkout not present (GPU box)")
 def test_config_defaults_equal_the_live_reference_config():
-    """exec the reference's own class (configuration_dreamllm.py:64-278) on the installed transformers and compare every default."""
-    from transformers import PretrainedConfig
-
-    class _Log:
-        def warning(self, *a, **k):
-            pass
-        info = warning
-
-    src = open(REF_CFG).read().split("\n")
-    ns = dict(PretrainedConfig=PretrainedConfig, logger=_Log(), CLASS_KEY="_class_", NAME_KEY="_name_", PLUGIN_TYPE_KEY="_plugin_type_")
-    exec("from __future__ import annotations\n" + "\n".join(src[63:278]), ns)
-    ref, ours = ns["DreamLLMConfig"](), DreamLLMConfig()
-    for k, v in ours.to_dict().items():
-        if k in ("model_type", "rope_scaling"):            # transformers 5 rewrites rope_scaling=None into rope_parameters
-            continue
-        assert getattr(ref, k) == v, k
-    assert ref.model_type == ours.model_type == "dreamllm"
+    """Every default of the reference's own `DreamLLMConfig` (configuration_dreamllm.py:64-278, exec'd on transformers by
+    oracle/gen_golden_surface.py and stored in tests/golden/reference_config.json) equals ours, and so does its special-token table."""
+    ref = json.load(open(REF_CFG))
+    ours = DreamLLMConfig()
+    mine = {k: v for k, v in ours.to_dict().items()
+            if k not in ("model_type", "rope_scaling")}    # transformers 5 rewrites rope_scaling=None into rope_parameters
+    assert set(mine) == set(ref["defaults"])
+    for k, v in mine.items():
+        assert ref["defaults"][k] == json.loads(json.dumps(v, default=str)), k
+    assert ref["model_type"] == ours.model_type == "dreamllm"
     tok = Tok(96)
     tokens = {"additional_special_tokens": ["<im_start>", "<dream_start>"], "bos_token": "<s>"}
-    ref.update_special_tokens2ids_dict(tokens, tok)
     ours.update_special_tokens2ids_dict(tokens, tok)
-    assert ref.special_tokens2ids_dict == ours.special_tokens2ids_dict == {"additional_special_tokens": {"<im_start>": 90, "<dream_start>": 93},
-                                                                           "<s>": 1}
+    assert ref["special_tokens2ids_dict"] == ours.special_tokens2ids_dict == {"additional_special_tokens": {"<im_start>": 90,
+                                                                                                           "<dream_start>": 93}, "<s>": 1}
 
 
 def test_plugin_registration_and_instantiation():

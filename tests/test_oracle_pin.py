@@ -1,7 +1,6 @@
 """Pin the CPU oracle (oracle/decoder_oracle.py) to the reference.
 
-(a) against tests/golden/*.npz minted from the reference's own code (oracle/gen_golden.py);
-(b) against the live reference when /root/reference exists (build container only).
+against tests/golden/*.npz minted from the reference's own code (oracle/gen_golden.py, oracle/gen_golden_bf16.py).
 """
 import glob
 import os
@@ -11,9 +10,10 @@ import pytest
 import torch
 
 from oracle import decoder_oracle as O
-from oracle import gen_golden, ref_exec
+from oracle import gen_golden, gen_golden_bf16
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "decoder_layer_*.npz")))
+BF16_PINS = os.path.join(os.path.dirname(__file__), "golden", "bf16_pins.npz")
 
 
 def _run_oracle(hidden, inter, heads, bsz, seq, seed, pad):
@@ -60,28 +60,24 @@ def test_golden_present():
     assert len(GOLDEN) >= 3
 
 
-@pytest.mark.skipif(not ref_exec.available(), reason="/root/reference only exists in the build container")
+def _bf16(bits):
+    return torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16)
+
+
 def test_oracle_matches_live_reference_bf16_rounding_points():
-    """bf16 run: the oracle must share the reference's rounding points (norm cast before the
-    weight multiply, bf16 rope tables, fp32 softmax) — compare bit-for-bit-ish in bf16."""
-    ns = ref_exec.load_reference_namespace()
-    hidden, inter, heads, bsz, seq, seed = 256, 512, 2, 2, 40, 5
-    cfg = ref_exec.make_config(hidden, inter, heads)
-    layer = ns["DreamLLMDecoderLayer"](cfg).float()
+    """bf16 run: the oracle must share the reference's rounding points (norm cast before the weight multiply, bf16 rope tables, fp32
+    softmax) — bit for bit against the reference layer's bf16 output stored in tests/golden/bf16_pins.npz (oracle/gen_golden_bf16.py)."""
+    g = np.load(BF16_PINS)
+    hidden, inter, heads, bsz, seq, seed = gen_golden_bf16.LAYER_CASE
     p = O.init_layer_params(hidden, inter, seed)
-    sd = dict(p)
-    sd["self_attn.rotary_emb.inv_freq"] = layer.self_attn.rotary_emb.inv_freq
-    layer.load_state_dict(sd)
-    layer = layer.to(torch.bfloat16)
     x, _ = gen_golden.make_inputs(hidden, bsz, seq, seed)
     xb = x.to(torch.bfloat16)
     pos = torch.arange(seq)[None].expand(bsz, -1)
-    y_ref = layer(xb, attention_mask=ref_exec.causal_mask_4d(bsz, seq, torch.bfloat16), position_ids=pos)[0]
     pb = {k: v.to(torch.bfloat16) for k, v in p.items()}
     # reference casts the fp32-built tables to the activation dtype at use (:126-127)
     cos, sin = O.rope_tables(hidden // heads, 2048, dtype=torch.bfloat16)
     y = O.decoder_layer(xb, pb, heads, cos, sin, pos, O.causal_additive_mask(bsz, seq, torch.bfloat16))
-    assert torch.equal(y, y_ref)
+    assert torch.equal(y, _bf16(g["layer_y"]))
 
 
 def test_lm_loss_masked_mean():
@@ -111,25 +107,14 @@ def test_kvcache_oracle_matches_reference_golden():
     # pad QUERY rows differ by design between the reference's two paths (SURVEY §8 row a3'): eager = uniform attention, flash = zeros
 
 
-@pytest.mark.skipif(not ref_exec.available(), reason="/root/reference only exists in the build container")
 def test_kvcache_oracle_matches_live_reference_bf16():
-    """Same scenario, bf16, against the live reference: shared rounding points => identical outputs on the valid rows."""
-    from transformers.modeling_attn_mask_utils import _prepare_4d_causal_attention_mask
-    BF = torch.bfloat16
-    hidden, inter, heads = 256, 512, 2
+    """Same scenario, bf16, against the reference's own `past_key_value` path run in bf16 (tests/golden/bf16_pins.npz): shared rounding
+    points => identical outputs on the valid rows."""
+    g = np.load(BF16_PINS)
+    hidden, inter, heads = gen_golden_bf16.KV_CASE
     p, calls = O.cached_decode_scenario(hidden, inter, heads)
-    ns = ref_exec.load_reference_namespace()
-    layer = ns["DreamLLMDecoderLayer"](ref_exec.make_config(hidden, inter, heads)).float()
-    sd = {k: v.clone() for k, v in p.items()}
-    sd["self_attn.rotary_emb.inv_freq"] = layer.self_attn.rotary_emb.inv_freq.clone()
-    layer.load_state_dict(sd)
-    layer = layer.to(BF)
-    outs = O.run_cached_scenario(p, calls, heads, dtype=BF)
-    past = None
-    with torch.no_grad():
-        for (x, am, pos), y in zip(calls, outs):
-            past_len = 0 if past is None else past[0].shape[2]
-            mask = _prepare_4d_causal_attention_mask(am, (x.shape[0], x.shape[1]), x.to(BF), past_len)
-            yr, past = layer(x.to(BF), attention_mask=mask, position_ids=pos, past_key_value=past, use_cache=True)
-            valid = am[:, -x.shape[1]:].bool()
-            assert torch.equal(yr[valid], y[valid])
+    outs = O.run_cached_scenario(p, calls, heads, dtype=torch.bfloat16)
+    assert len(outs) == 4
+    for i, ((x, am, pos), y) in enumerate(zip(calls, outs)):
+        valid = am[:, -x.shape[1]:].bool()
+        assert torch.equal(_bf16(g[f"kv_y{i}"])[valid], y[valid]), f"call {i}"
