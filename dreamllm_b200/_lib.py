@@ -99,6 +99,7 @@ SIGNATURES = {
     "dllm_conv_in": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "dllm_conv_out": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "dllm_gemm_splitk_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dllm_gemm_tile_n": (_i, [_i, _i, _i, _i]),
     "dllm_gemm_bf16_ws": (_i, [_vp, _vp, _vp, _i, _i, _i, _l, _l, _l, _i, _vp, _vp, _l, _i, _vp, _sz, _vp]),
     "dllm_conv3x3_splitk_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "dllm_conv3x3_nhwc_ws": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),

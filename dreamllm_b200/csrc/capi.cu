@@ -196,6 +196,7 @@ int dllm_conv_out(const void* x, const void* w, const void* bias, float* y, int 
   return conv_out_nhwc_to_nchw(x, w, bias, y, B, C, H, W, Cout, S(stream));
 }
 size_t dllm_gemm_splitk_workspace_bytes(int M, int N, int K) { return gemm_splitk_workspace(M, N, K); }
+int dllm_gemm_tile_n(int M, int N, int K, int b_mn) { return gemm_tile_bn(M, N, K, b_mn); }
 int dllm_gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int b_mn, const void* bias,
                       const void* residual, long ldr, int act, void* ws, size_t ws_bytes, void* stream) {
   ensure_context(A);

@@ -24,7 +24,7 @@
 namespace dllm {
 
 constexpr int BM = 128;  // A rows per CTA (two consumer warpgroups x 64)
-constexpr int BN = 256;  // default N tile (kBN = 128 is instantiated for outputs whose width tiles badly by 256: see pick_bn)
+constexpr int BN = 256;  // widest N tile (kBN 128 / 160 / 192 / 224 are instantiated for outputs whose width tiles badly by 256: see plan_bn)
 constexpr int BK = 64;   // 64 bf16 = one 128-byte swizzle line
 constexpr int kGemmThreads = 384;
 
@@ -34,7 +34,8 @@ struct GemmCfg {
   static constexpr int kBBytes = kBN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kBarBytes = 256;
-  // operand stages + barriers <= 227 KB:  kBN 256: 4 stages, kBN 128: 7
+  // operand stages + barriers <= 227 KB:  kBN 256: 4 stages, 224 / 192: 5, 160: 6, 128: 7 (every stage size is a multiple of the
+  // 1 KB the 128-byte swizzle needs as alignment)
   static constexpr int kStagesFit = (227 * 1024 - kBarBytes - 1024) / kStageBytes;
   static constexpr int kStages = kStagesFit > 8 ? 8 : kStagesFit;
   static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024 /*align slack*/;
@@ -364,9 +365,52 @@ int num_sms() {
   return n;
 }
 
-// N-tile width: 256 (the widest wgmma, half the A re-reads from shared memory per MMA of a 128-wide tile) except for outputs that fit
-// ONE 128-wide tile, where a 256-wide tile would be half padding.
+// N-tile width of split-K launches (plan_split) and of the launches that have no intermediate width (MN-major A, fp32 out): 256 (the
+// widest wgmma, half the A re-reads from shared memory per MMA of a 128-wide tile) except for outputs that fit ONE 128-wide tile, where a
+// 256-wide tile would be half padding.
 static inline int pick_bn(int N) { return N <= 128 ? 128 : 256; }
+
+// Tile planner of the unsplit bf16-output launches with K-major A (forward NT, dgrad NN, conv): the N width that minimises
+// ceil(tiles / SMs) x t(width), t being the per-tile time relative to 256 (DESIGN §4 has the measurement).  A width that fits N exactly
+// computes no padding columns (UNet C = 320 / 640 / 960), and a narrower tile can fill the last wave of a small-M launch (LLM M = 400).
+// MN-major B is fetched in 64-column boxes, so its widths are multiples of 64.  t varies by about +-15 % from shape to shape, so costs
+// within 5 % of the least count as a tie, and ties go to the wider tile (widest first below): on many-wave launches (7B training at
+// 8192 tokens) the wave counts of all widths come out nearly even and 256, the most efficient per column, stays.
+struct BnCost {
+  int bn;
+  float t;
+};
+static constexpr BnCost kBnKMajor[] = {{256, 1.f}, {224, 0.861f}, {192, 0.781f}, {160, 0.645f}, {128, 0.536f}};
+static constexpr BnCost kBnMNMajor[] = {{256, 1.f}, {192, 0.781f}, {128, 0.536f}};
+
+// DLLM_GEMM_BN=<width> pins the planner's choice (scripts/gemm_shapes.py times every width this way); other widths are ignored.
+static int forced_bn() {
+  static const int bn = [] {
+    const char* s = getenv("DLLM_GEMM_BN");
+    return s ? atoi(s) : 0;
+  }();
+  return bn;
+}
+
+static int plan_bn(int M, int N, int a_mn, int b_mn, bool bf16_out) {
+  if (a_mn || !bf16_out) return pick_bn(N);
+  const BnCost* w = b_mn ? kBnMNMajor : kBnKMajor;
+  const int nw = b_mn ? sizeof(kBnMNMajor) / sizeof(BnCost) : sizeof(kBnKMajor) / sizeof(BnCost);
+  for (int i = 0; i < nw; ++i)
+    if (w[i].bn == forced_bn()) return w[i].bn;
+  int slots = num_sms() - g_reserved_sms;
+  if (slots < 1) slots = 1;
+  const long mt = (M + BM - 1) / BM;
+  float cost[8], least = 0.f;
+  for (int i = 0; i < nw; ++i) {
+    const long tiles = mt * ((N + w[i].bn - 1) / w[i].bn);
+    cost[i] = static_cast<float>((tiles + slots - 1) / slots) * w[i].t;
+    if (i == 0 || cost[i] < least) least = cost[i];
+  }
+  for (int i = 0; i < nw; ++i)
+    if (cost[i] <= 1.05f * least) return w[i].bn;
+  return w[0].bn;
+}
 
 template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN>
 static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
@@ -386,12 +430,20 @@ static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, void* C,
   kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, static_cast<OutT*>(C), ldc, M, N, K, 16, epi, cg, ksplit);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
-// `bn` must be the value the B tensor map's box was built for (pick_bn(N))
+// `bn` must be the value the B tensor map's box was built for (plan_bn); only the widths plan_bn can return are instantiated
 template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
-                       cudaStream_t stream, ConvGeom cg = ConvGeom{1, 1, 1, 1}, int bn = BN) {
+                       cudaStream_t stream, ConvGeom cg, int bn) {
+  if constexpr (!kAMN && sizeof(OutT) == 2) {
+    if (bn == 192) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 192>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+    if constexpr (!kBMN) {
+      if (bn == 160) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 160>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+      if (bn == 224) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 224>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+    }
+  }
   if (bn == 128) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 128>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
-  return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 256>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  if (bn == 256) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 256>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  return DLLM_ERR_UNSUPPORTED;
 }
 
 // ------------------------------------------------------------------------------------------------ split-K (small-M shapes)
@@ -425,6 +477,10 @@ static SplitPlan plan_split(int M, int N, int K) {
   return p;
 }
 size_t gemm_splitk_workspace(int M, int N, int K) { return plan_split(M, N, K).ws_bytes; }
+int gemm_tile_bn(int M, int N, int K, int b_mn) {
+  const SplitPlan p = plan_split(M, N, K);
+  return p.ksplit > 1 ? p.bn : plan_bn(M, N, 0, b_mn, true);
+}
 
 // out[m, n] = epilogue( sum_ks ws[ks * mp + m, n] ): bias / row-group bias added in fp32, rounded to bf16, optional activation (rounded),
 // optional residual add (rounded) — the rounding points of gemm_kernel's fused epilogues.  One thread = 8 columns.
@@ -517,7 +573,7 @@ int gemm_bf16_ex(const void* A, const void* B, void* C, int M, int N, int K, lon
   if (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) return DLLM_ERR_ALIGN;
   if (reinterpret_cast<uintptr_t>(C) & 15) return DLLM_ERR_ALIGN;
   GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), ldr, act, nullptr, 1};
-  const int bn = pick_bn(N);
+  const int bn = plan_bn(M, N, a_mn, b_mn, !out_fp32);
   const ConvGeom nocg{1, 1, 1, 1};
   CUtensorMap ta, tb;
   int rc;
@@ -606,15 +662,16 @@ int conv3x3_nhwc_ws(const void* x, const void* w, void* y, int Nimg, int H, int 
     return DLLM_ERR_SHAPE;
   }
   const int M = Nimg * HW, K = 9 * Cin;
-  const int bn = pick_bn(Cout);
+  const SplitPlan sp = plan_split(M, Cout, K);
+  const bool split = sp.ksplit > 1 && ws && ws_bytes >= sp.ws_bytes && !(reinterpret_cast<uintptr_t>(ws) & 15);
+  const int bn = split ? sp.bn : plan_bn(M, Cout, 0, 0, true);
   CUtensorMap ta, tb;
   int rc;
   if ((rc = make_tmap_nhwc(&ta, x, Nimg, H, W, Cin, Wb, Hb, Nb))) return rc;
   if ((rc = make_tmap_2d(&tb, w, 2, Cout, K, K, bn, BK))) return rc;
   GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), Cout, 0, static_cast<const bf16*>(rowbias), HW};
   ConvGeom cg{Cin / 64, W, H, HW};
-  const SplitPlan sp = plan_split(M, Cout, K);
-  if (sp.ksplit > 1 && ws && ws_bytes >= sp.ws_bytes && !(reinterpret_cast<uintptr_t>(ws) & 15)) {
+  if (split) {
     GemmEpi none{nullptr, nullptr, 0, 0, nullptr, 1};
     rc = (bn == 128) ? launch_gemm_bn<false, false, float, true, 0, 128>(ta, tb, ws, Cout, M, Cout, K, none, stream, cg, sp.ksplit)
                      : launch_gemm_bn<false, false, float, true, 0, 256>(ta, tb, ws, Cout, M, Cout, K, none, stream, cg, sp.ksplit);

@@ -31,6 +31,8 @@ int gemm_bf16_ex(const void* A, const void* B, void* C, int M, int N, int K, lon
 
 // split-K variants for small-M shapes (workspace sized by the *_workspace query; 0 = the shape is not split)
 size_t gemm_splitk_workspace(int M, int N, int K);
+// N-tile width a bf16-output GEMM with K-major A uses when run with that workspace: the split-K width, or the tile planner's
+int gemm_tile_bn(int M, int N, int K, int b_mn);
 int gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int b_mn, const void* bias,
                  const void* residual, long ldr, int act, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t conv3x3_splitk_workspace(int Nimg, int H, int W, int Cin, int Cout);

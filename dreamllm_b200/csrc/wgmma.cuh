@@ -59,6 +59,51 @@ template <int kTA, int kTB> struct WgmmaSS<256, kTA, kTB> {
   }
 };
 
+// The intermediate GEMM tile widths (gemm_sm90.cu's tile planner).  Their operand lists are built from decades of accumulator operands:
+// DLLM_ACC_S10(t) is the template text "%t0, ..., %t9" (t empty: "%0, ..., %9") and DLLM_ACC_F10(i) the constraints of d[i .. i + 9].
+#define DLLM_ACC_S2(t) "%" #t "0, %" #t "1"
+#define DLLM_ACC_S6(t) DLLM_ACC_S2(t) ", %" #t "2, %" #t "3, %" #t "4, %" #t "5"
+#define DLLM_ACC_S10(t) DLLM_ACC_S6(t) ", %" #t "6, %" #t "7, %" #t "8, %" #t "9"
+#define DLLM_ACC_F2(i) "+f"(d[(i)]), "+f"(d[(i) + 1])
+#define DLLM_ACC_F6(i) DLLM_ACC_F2(i), DLLM_ACC_F2((i) + 2), DLLM_ACC_F2((i) + 4)
+#define DLLM_ACC_F10(i) DLLM_ACC_F6(i), DLLM_ACC_F2((i) + 6), DLLM_ACC_F2((i) + 8)
+#define DLLM_ACC_S80 DLLM_ACC_S10() ", " DLLM_ACC_S10(1) ", " DLLM_ACC_S10(2) ", " DLLM_ACC_S10(3) ", " DLLM_ACC_S10(4) ", " \
+                     DLLM_ACC_S10(5) ", " DLLM_ACC_S10(6) ", " DLLM_ACC_S10(7)
+#define DLLM_ACC_F80 DLLM_ACC_F10(0), DLLM_ACC_F10(10), DLLM_ACC_F10(20), DLLM_ACC_F10(30), DLLM_ACC_F10(40), DLLM_ACC_F10(50), \
+                     DLLM_ACC_F10(60), DLLM_ACC_F10(70)
+#define DLLM_ACC_S90 DLLM_ACC_S80 ", " DLLM_ACC_S10(8)
+#define DLLM_ACC_F90 DLLM_ACC_F80, DLLM_ACC_F10(80)
+#define DLLM_ACC_S110 DLLM_ACC_S90 ", " DLLM_ACC_S10(9) ", " DLLM_ACC_S10(10)
+#define DLLM_ACC_F110 DLLM_ACC_F90, DLLM_ACC_F10(90), DLLM_ACC_F10(100)
+
+template <int kTA, int kTB> struct WgmmaSS<160, kTA, kTB> {
+  static __device__ __forceinline__ void run(float* d, uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 {" DLLM_ACC_S80 "}, %80, %81, p, 1, 1, %83, %84;\n}\n"
+        : DLLM_ACC_F80
+        : "l"(da), "l"(db), "r"(acc), "n"(kTA), "n"(kTB));
+  }
+};
+template <int kTA, int kTB> struct WgmmaSS<192, kTA, kTB> {
+  static __device__ __forceinline__ void run(float* d, uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 {" DLLM_ACC_S90 ", " DLLM_ACC_S6(9) "}, %96, %97, p, 1, 1, %99, %100;\n}\n"
+        : DLLM_ACC_F90, DLLM_ACC_F6(90)
+        : "l"(da), "l"(db), "r"(acc), "n"(kTA), "n"(kTB));
+  }
+};
+template <int kTA, int kTB> struct WgmmaSS<224, kTA, kTB> {
+  static __device__ __forceinline__ void run(float* d, uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n224k16.f32.bf16.bf16 {" DLLM_ACC_S110 ", " DLLM_ACC_S2(11) "}, %112, %113, p, 1, 1, %115, %116;\n}\n"
+        : DLLM_ACC_F110, DLLM_ACC_F2(110)
+        : "l"(da), "l"(db), "r"(acc), "n"(kTA), "n"(kTB));
+  }
+};
+
 template <int N, int kTA, int kTB>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, int acc) { WgmmaSS<N, kTA, kTB>::run(d, da, db, acc); }
 template <int N, int kTB>

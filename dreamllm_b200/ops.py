@@ -29,7 +29,8 @@ class _LaunchCounter:
 
 
 class _GemmProfile:
-    """Optional live CUDA-event timing of every GEMM launch on the launching stream (bench.py roofline)."""
+    """Optional live CUDA-event timing of every GEMM and implicit-GEMM conv launch on the launching stream (bench.py roofline).
+    A record is (start event, end event, FLOPs, (M, N, K, mode)); mode is fwd / dgrad / wgrad / tn, geglu or conv3x3."""
 
     def __init__(self):
         self.enabled = False
@@ -39,11 +40,32 @@ class _GemmProfile:
         self.enabled = enabled
         self.records = []
 
+    def start(self):
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+        return e0
+
+    def stop(self, e0, flops, key):
+        e1 = torch.cuda.Event(enable_timing=True)
+        e1.record()
+        self.records.append((e0, e1, flops, key))
+
     def summary(self):
         torch.cuda.synchronize()
-        ms = sum(s.elapsed_time(e) for s, e, _ in self.records)
-        fl = sum(f for _, _, f in self.records)
+        ms = sum(s.elapsed_time(e) for s, e, _, _ in self.records)
+        fl = sum(f for _, _, f, _ in self.records)
         return {"ms": ms, "tflops": (fl / 1e9 / ms) if ms > 0 else None, "n": len(self.records)}
+
+    def by_shape(self):
+        """{(M, N, K, mode): [launches, ms, FLOPs]} over the records."""
+        torch.cuda.synchronize()
+        out = {}
+        for s, e, f, key in self.records:
+            r = out.setdefault(key, [0, 0.0, 0.0])
+            r[0] += 1
+            r[1] += s.elapsed_time(e)
+            r[2] += f
+        return out
 
 
 LAUNCHES = _LaunchCounter()
@@ -93,8 +115,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         out = torch.empty((M, N), device=a.device, dtype=out_dtype)
     assert out.shape == (M, N) and out.stride(1) == 1 and out.dtype in (BF16, torch.float32)
     if PROFILE.enabled:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
+        e0 = PROFILE.start()
     wsb = 0
     if not a_mn and out.dtype == BF16 and cta_pair < 0 and M <= 4096:          # small-M shapes: split-K when the library says it pays
         wsb = lib().dllm_gemm_splitk_workspace_bytes(M, N, K)
@@ -126,8 +147,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
                                      int(act), _stream())
     check(rc, "dllm_gemm_bf16")
     if PROFILE.enabled:
-        e1.record()
-        PROFILE.records.append((e0, e1, 2.0 * M * N * K))
+        PROFILE.stop(e0, 2.0 * M * N * K, (M, N, K, (("tn", "wgrad") if a_mn else ("fwd", "dgrad"))[int(b_mn)]))
     LAUNCHES.add(1)
     return out
 
@@ -158,13 +178,11 @@ def linear_geglu(x2d: torch.Tensor, w_perm: torch.Tensor, b_perm: torch.Tensor |
     assert x2d.dtype == BF16 and w_perm.dtype == BF16 and x2d.stride(1) == 1 and w_perm.is_contiguous() and w_perm.shape[1] == K
     out = torch.empty((M, N // 2), device=x2d.device, dtype=BF16)
     if PROFILE.enabled:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
+        e0 = PROFILE.start()
     check(lib().dllm_gemm_bf16_geglu(_p(x2d), _p(w_perm), _p(b_perm), _p(out), M, N, K, x2d.stride(0), w_perm.stride(0), out.stride(0),
                                      _stream()), "dllm_gemm_bf16_geglu")
     if PROFILE.enabled:
-        e1.record()
-        PROFILE.records.append((e0, e1, 2.0 * M * N * K))
+        PROFILE.stop(e0, 2.0 * M * N * K, (M, N, K, "geglu"))
     LAUNCHES.add(1)
     return out
 
@@ -416,16 +434,20 @@ def conv3x3(x_nhwc, w_k, bias=None, rowbias=None, residual=None):
         assert residual.is_contiguous() and residual.numel() == y.numel()
     if rowbias is not None:
         assert rowbias.is_contiguous() and rowbias.shape == (N, Cout)
+    if PROFILE.enabled:
+        e0 = PROFILE.start()
     wsb = lib().dllm_conv3x3_splitk_workspace_bytes(N, H, W, Cin, Cout) if N * H * W <= 4096 else 0
     if wsb:                                                    # small planes (8x8 / 16x16 of a few samples): split-K + reduce
         ws = torch.empty(wsb, device=x_nhwc.device, dtype=torch.uint8)
         check(lib().dllm_conv3x3_nhwc_ws(_p(x_nhwc), _p(w_k), _p(y), N, H, W, Cin, Cout, _p(bias), _p(rowbias), _p(residual), _p(ws), wsb,
                                          _stream()), "dllm_conv3x3_nhwc_ws")
         LAUNCHES.add(2)
-        return y
-    check(lib().dllm_conv3x3_nhwc(_p(x_nhwc), _p(w_k), _p(y), N, H, W, Cin, Cout, _p(bias), _p(rowbias), _p(residual), _stream()),
-          "dllm_conv3x3_nhwc")
-    LAUNCHES.add(1)
+    else:
+        check(lib().dllm_conv3x3_nhwc(_p(x_nhwc), _p(w_k), _p(y), N, H, W, Cin, Cout, _p(bias), _p(rowbias), _p(residual), _stream()),
+              "dllm_conv3x3_nhwc")
+        LAUNCHES.add(1)
+    if PROFILE.enabled:
+        PROFILE.stop(e0, 2.0 * N * H * W * Cout * 9 * Cin, (N * H * W, Cout, 9 * Cin, "conv3x3"))
     return y
 
 

@@ -143,6 +143,9 @@ int dllm_conv_out(const void* x_nhwc, const void* w, const void* bias, float* y_
  * the GEMM writes fp32 K-slice partials there and a reduce kernel applies bias / row-group bias / activation / residual with the fused
  * epilogue's rounding points.  C = act(bf16(A B^T + bias)) (+ residual) for b_mn = 0 (nn.Linear forward), C = A B for b_mn = 1 (dgrad). */
 size_t dllm_gemm_splitk_workspace_bytes(int M, int N, int K);
+/* N-tile width (128, 160, 192, 224 or 256) that dllm_gemm_bf16_ws uses for this shape when given its workspace: the split-K width when
+ * the shape is split, otherwise the width the tile planner picks (b_mn = 1 is the dgrad NN form).  Pure host code. */
+int dllm_gemm_tile_n(int M, int N, int K, int b_mn);
 int dllm_gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int b_mn, const void* bias,
                       const void* residual, long ldr, int act, void* ws, size_t ws_bytes, void* stream);
 size_t dllm_conv3x3_splitk_workspace_bytes(int N, int H, int W, int Cin, int Cout);
