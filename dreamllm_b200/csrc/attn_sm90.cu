@@ -10,6 +10,8 @@
 //     S / dP come from two shared-memory operands, P / dS are fed to the next wgmma straight from registers (the m64nN accumulator
 //     fragment of a 16-column slice is the m64k16 A-operand fragment, so no shuffle or shared-memory round trip is needed);
 //   * the ring stage of tile j is refilled with tile j + 2 once both warpgroups have passed the CTA barrier at the end of iteration j.
+// Grouped-query attention: k/v carry nkv = nh / group heads and q head h reads kv head h / group (reference repeat_kv, :242-252).  The
+// forward and dQ kernels only remap the K/V column they load; the dK/dV kernel runs one CTA per kv head and sums the group's q heads.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -107,7 +109,7 @@ template <int D, bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                 const __grid_constant__ CUtensorMap tv, bf16* __restrict__ out, long ld_o, float* __restrict__ lse,
-                const int* __restrict__ seqlens, int S, int Skv, int nh, float scale_log2,
+                const int* __restrict__ seqlens, int S, int Skv, int nh, int group, float scale_log2,
                 const uint8_t* __restrict__ kv_mask, int mask_ld) {
   // kv_mask (nullable): [B, mask_ld] bytes, 0 = padded key position that no query may attend to — the 2-D `attention_mask` of a padded
   // batch living inside a kv-cache (reference :553-583 drops those tokens with `_upad_input`; HF left-pads decoder-only prompts)
@@ -124,6 +126,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
 
   // causal: q tile i has i + 1 KV tiles of work; launch the heaviest first so the grid's tail is made of short CTAs (LPT order)
   const int q0 = (kCausal ? (gridDim.x - 1 - blockIdx.x) : blockIdx.x) * 128, h = blockIdx.y, b = blockIdx.z;
+  const int hkv = h / group;
   const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;   // Skv != S only for cross-attention (non-causal)
   const int q_len = seqlens ? kv_len : S;                    // right-padded self-attention: rows >= len are padding
   const int kv_end = kCausal ? min(kv_len, q0 + 128 + coff) : kv_len;
@@ -140,8 +143,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     const int st = j & 1;
     mbar_arrive_expect_tx(&kv_full[st], 2 * kBKV * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + st * L::kKV + c * kBKV * 128, &tk, &kv_full[st], h * D + c * 64, j * kBKV, b);
-      tma_load_3d(smem + L::oV + st * L::kKV + c * kBKV * 128, &tv, &kv_full[st], h * D + c * 64, j * kBKV, b);
+      tma_load_3d(smem + L::oK + st * L::kKV + c * kBKV * 128, &tk, &kv_full[st], hkv * D + c * 64, j * kBKV, b);
+      tma_load_3d(smem + L::oV + st * L::kKV + c * kBKV * 128, &tv, &kv_full[st], hkv * D + c * 64, j * kBKV, b);
     }
   };
   if (threadIdx.x == 0 && n_kv > 0) {
@@ -305,9 +308,11 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const bf16* __restri
 }
 
 // ================================================================================================ backward: dK, dV
-// CTA = one 128-row kv tile of one (b, h) (64 kv rows per warpgroup); 64-row q tiles (Q and dO) stream through the ring.
+// CTA = one 128-row kv tile of one (b, kv head hk) (64 kv rows per warpgroup); 64-row q tiles (Q and dO) stream through the ring.
 //   S^T = K Q^T, dP^T = V dO^T (both operands from shared memory), P^T = exp2(S^T * scale log2e - lse2[q]), dS^T = P^T (dP^T - delta[q]),
 //   dV += P^T dO and dK += dS^T Q with P^T / dS^T as register A operands and dO / Q read MN-major.
+// Under GQA the CTA walks the flattened sequence (q head hk * group + g) x (q tile i), g outer, and keeps summing into the same register
+// accumulators: the group's sum has one fixed order (no atomics, no workspace), and the ring runs on across head boundaries.
 template <int D>
 struct BwdKVSmem {
   static constexpr int NCH = D / 64;
@@ -322,7 +327,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                      const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, bf16* __restrict__ dk,
                      bf16* __restrict__ dv, long ld_dkv, const float* __restrict__ lse2, const float* __restrict__ delta,
-                     const int* __restrict__ seqlens, int S, int Skv, int Sp, int nh, float scale, float scale_log2) {
+                     const int* __restrict__ seqlens, int S, int Skv, int Sp, int nh, int group, float scale, float scale_log2) {
   using L = BwdKVSmem<D>;
   constexpr int NCH = L::NCH;
   extern __shared__ uint8_t smem_raw[];
@@ -330,12 +335,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
   uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + L::oBar);
   uint64_t* q_full = kv_full + 1;                 // [2]
 
-  const int kv0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
+  const int kv0 = blockIdx.x * 128, hk = blockIdx.y, b = blockIdx.z;
   const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;
   const int q_len = seqlens ? kv_len : S;
   const int i0 = kCausal ? kv0 / 64 : 0;           // first q tile that can see this kv tile
   const int i1 = (kv0 < kv_len) ? (q_len + 63) / 64 : 0;
   const int n_q = max(0, i1 - i0);
+  const int n_items = n_q * group;                 // item it = (q head hk * group + it / n_q, q tile i0 + it % n_q)
 
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
@@ -344,37 +350,37 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     fence_mbar_init();
   }
   __syncthreads();
-  auto load_q = [&](int i) {
-    const int st = (i - i0) & 1;
+  auto load_q = [&](int it) {
+    const int st = it & 1, g = it / n_q, i = i0 + (it - g * n_q), col = (hk * group + g) * D;
     mbar_arrive_expect_tx(&q_full[st], 2 * 64 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oQ + st * L::kQT + c * 8192, &tq, &q_full[st], h * D + c * 64, i * 64, b);
-      tma_load_3d(smem + L::oDO + st * L::kQT + c * 8192, &tdo, &q_full[st], h * D + c * 64, i * 64, b);
+      tma_load_3d(smem + L::oQ + st * L::kQT + c * 8192, &tq, &q_full[st], col + c * 64, i * 64, b);
+      tma_load_3d(smem + L::oDO + st * L::kQT + c * 8192, &tdo, &q_full[st], col + c * 64, i * 64, b);
     }
   };
-  if (threadIdx.x == 0 && n_q > 0) {
+  if (threadIdx.x == 0 && n_items > 0) {
     mbar_arrive_expect_tx(kv_full, 2 * 128 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + c * 16384, &tk, kv_full, h * D + c * 64, kv0, b);
-      tma_load_3d(smem + L::oV + c * 16384, &tv, kv_full, h * D + c * 64, kv0, b);
+      tma_load_3d(smem + L::oK + c * 16384, &tk, kv_full, hk * D + c * 64, kv0, b);
+      tma_load_3d(smem + L::oV + c * 16384, &tv, kv_full, hk * D + c * 64, kv0, b);
     }
-    load_q(i0);
-    if (n_q > 1) load_q(i0 + 1);
+    load_q(0);
+    if (n_items > 1) load_q(1);
   }
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c_in = 2 * (t & 3);
   const int row_t = kv0 + wg * 64 + r_in;          // kv row of accumulator element (h = 0); + 8 for h = 1
   const uint32_t sK = smem_u32(smem + L::oK) + wg * 8192, sV = smem_u32(smem + L::oV) + wg * 8192;
-  const float* lse_bh = lse2 + (static_cast<size_t>(b) * nh + h) * Sp;
-  const float* del_bh = delta + (static_cast<size_t>(b) * nh + h) * Sp;
   float dka[D / 2], dva[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dka[i] = dva[i] = 0.f;
-  if (n_q > 0) mbar_wait(kv_full, 0, 3);
-  for (int i = i0; i < i0 + n_q; ++i) {
-    const int st = (i - i0) & 1;
-    mbar_wait(&q_full[st], ((i - i0) >> 1) & 1, 4);
+  if (n_items > 0) mbar_wait(kv_full, 0, 3);
+  for (int it = 0; it < n_items; ++it) {
+    const int st = it & 1, g = it / n_q, i = i0 + (it - g * n_q);
+    const float* lse_bh = lse2 + (static_cast<size_t>(b) * nh + hk * group + g) * Sp;
+    const float* del_bh = delta + (static_cast<size_t>(b) * nh + hk * group + g) * Sp;
+    mbar_wait(&q_full[st], (it >> 1) & 1, 4);
     const uint32_t sQ = smem_u32(smem + L::oQ + st * L::kQT), sDO = smem_u32(smem + L::oDO + st * L::kQT);
     float sa[32], dpa[32];
     wgmma_fence();
@@ -413,11 +419,11 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     wgmma_commit();
     wgmma_wait<0>();
     __syncthreads();                                   // both warpgroups are done with ring stage st
-    if (threadIdx.x == 0 && i + 2 < i0 + n_q) load_q(i + 2);
+    if (threadIdx.x == 0 && it + 2 < n_items) load_q(it + 2);
   }
   const float ms[2] = {scale, scale}, one[2] = {1.f, 1.f};
-  store_rows<D>(dka, dk, ld_dkv, b, Skv, row_t, h * D, c_in, ms);
-  store_rows<D>(dva, dv, ld_dkv, b, Skv, row_t, h * D, c_in, one);
+  store_rows<D>(dka, dk, ld_dkv, b, Skv, row_t, hk * D, c_in, ms);
+  store_rows<D>(dva, dv, ld_dkv, b, Skv, row_t, hk * D, c_in, one);
 }
 
 // ================================================================================================ backward: dQ
@@ -437,7 +443,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                    const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, bf16* __restrict__ dq,
                    long ld_dq, const float* __restrict__ lse2, const float* __restrict__ delta, const int* __restrict__ seqlens,
-                   int S, int Skv, int Sp, int nh, float scale, float scale_log2) {
+                   int S, int Skv, int Sp, int nh, int group, float scale, float scale_log2) {
   using L = BwdQSmem<D>;
   constexpr int NCH = L::NCH;
   extern __shared__ uint8_t smem_raw[];
@@ -446,6 +452,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   uint64_t* kv_full = q_full + 1;                 // [2]
 
   const int q0 = (kCausal ? (gridDim.x - 1 - blockIdx.x) : blockIdx.x) * 128, h = blockIdx.y, b = blockIdx.z;
+  const int hkv = h / group;
   const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;
   const int q_len = seqlens ? kv_len : S;
   const int kv_end = (q0 < q_len) ? (kCausal ? min(kv_len, q0 + 128) : kv_len) : 0;
@@ -462,8 +469,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
     const int st = j & 1;
     mbar_arrive_expect_tx(&kv_full[st], 2 * 64 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + st * L::kKT + c * 8192, &tk, &kv_full[st], h * D + c * 64, j * 64, b);
-      tma_load_3d(smem + L::oV + st * L::kKT + c * 8192, &tv, &kv_full[st], h * D + c * 64, j * 64, b);
+      tma_load_3d(smem + L::oK + st * L::kKT + c * 8192, &tk, &kv_full[st], hkv * D + c * 64, j * 64, b);
+      tma_load_3d(smem + L::oV + st * L::kKT + c * 8192, &tv, &kv_full[st], hkv * D + c * 64, j * 64, b);
     }
   };
   if (threadIdx.x == 0 && n_kv > 0) {
@@ -544,8 +551,8 @@ static int set_smem(K kern, int bytes) {
 
 template <int D, bool C>
 static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, void* out, long ld_o, float* lse,
-                      const int* seqlens, int B, int S, int Skv, int nh, float scale_log2, cudaStream_t st, const uint8_t* kv_mask,
-                      int mask_ld) {
+                      const int* seqlens, int B, int S, int Skv, int nh, int group, float scale_log2, cudaStream_t st,
+                      const uint8_t* kv_mask, int mask_ld) {
   auto kern = attn_fwd_kernel<D, C>;
   static bool once = false;
   if (!once) {
@@ -553,27 +560,27 @@ static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
     once = true;
   }
   dim3 grid((S + 127) / 128, nh, B);
-  kern<<<grid, kAttnThreads, FwdSmem<D>::kBytes, st>>>(tq, tk, tv, static_cast<bf16*>(out), ld_o, lse, seqlens, S, Skv, nh, scale_log2,
-                                                       kv_mask, mask_ld);
+  kern<<<grid, kAttnThreads, FwdSmem<D>::kBytes, st>>>(tq, tk, tv, static_cast<bf16*>(out), ld_o, lse, seqlens, S, Skv, nh, group,
+                                                       scale_log2, kv_mask, mask_ld);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 
 int attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, int B, int S, int nh,
              int d, long ld_qkv, long ld_o, int causal, float scale, cudaStream_t st) {
-  return attn_fwd_ex(q, k, v, out, lse, seqlens, B, S, S, nh, d, ld_qkv, ld_qkv, ld_o, causal, scale, st);
+  return attn_fwd_gqa(q, k, v, out, lse, seqlens, nullptr, 0, B, S, S, S, nh, nh, d, ld_qkv, ld_qkv, ld_o, causal, scale, st);
 }
 
 // q: [B, S, nh, d] (token stride ld_q); k, v: [B, Skv, nh, d] (token stride ld_kv).  Skv != S = cross-attention.
 int attn_fwd_ex(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, int B, int S, int Skv,
                 int nh, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, cudaStream_t st) {
-  return attn_fwd_cache(q, k, v, out, lse, seqlens, B, S, Skv, Skv, nh, d, ld_q, ld_kv, ld_o, causal, scale, st);
+  return attn_fwd_gqa(q, k, v, out, lse, seqlens, nullptr, 0, B, S, Skv, Skv, nh, nh, d, ld_q, ld_kv, ld_o, causal, scale, st);
 }
 
 // kv_rows = rows allocated per batch entry in the k/v buffers (>= Skv): lets a preallocated kv-cache [B, max_len, nh*d] be read in
 // place with Skv valid rows.  causal with Skv > S uses the bottom-right aligned mask (decode / continuation).
 int attn_fwd_cache(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, int B, int S, int Skv,
                    int kv_rows, int nh, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, cudaStream_t st) {
-  return attn_fwd_cache_mask(q, k, v, out, lse, seqlens, nullptr, 0, B, S, Skv, kv_rows, nh, d, ld_q, ld_kv, ld_o, causal, scale, st);
+  return attn_fwd_gqa(q, k, v, out, lse, seqlens, nullptr, 0, B, S, Skv, kv_rows, nh, nh, d, ld_q, ld_kv, ld_o, causal, scale, st);
 }
 
 // + kv_mask [B, mask_ld] bytes (0 = padded key): a padded prompt batch inside the kv-cache.  mask_ld must cover whole 64-key tiles
@@ -581,7 +588,16 @@ int attn_fwd_cache(const void* q, const void* k, const void* v, void* out, float
 int attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
                         int mask_ld, int B, int S, int Skv, int kv_rows, int nh, int d, long ld_q, long ld_kv, long ld_o, int causal,
                         float scale, cudaStream_t st) {
+  return attn_fwd_gqa(q, k, v, out, lse, seqlens, kv_mask, mask_ld, B, S, Skv, kv_rows, nh, nh, d, ld_q, ld_kv, ld_o, causal, scale, st);
+}
+
+// The one forward entry every variant above funnels into.  k, v: [B, kv_rows, nkv, d] with nkv dividing nh (grouped-query attention;
+// nkv == nh is multi-head attention).
+int attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
+                 int mask_ld, int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
+                 float scale, cudaStream_t st) {
   if (B <= 0 || S <= 0 || Skv <= 0 || nh <= 0 || kv_rows < Skv) return DLLM_ERR_SHAPE;
+  if (nkv <= 0 || nh % nkv != 0) return DLLM_ERR_SHAPE;
   if (kv_mask && ((mask_ld & 15) || mask_ld < (Skv + 63) / 64 * 64 || (reinterpret_cast<uintptr_t>(kv_mask) & 15))) return DLLM_ERR_ALIGN;
   const uint8_t* km = static_cast<const uint8_t*>(kv_mask);
   if (d != 128 && d != 64) return DLLM_ERR_UNSUPPORTED;
@@ -591,13 +607,14 @@ int attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, 
   CUtensorMap tq, tk, tv;
   int rc;
   if ((rc = make_tmap_bsc(&tq, q, B, S, nh * d, ld_q, 128))) return rc;
-  if ((rc = make_tmap_bsc(&tk, k, B, kv_rows, nh * d, ld_kv, kBKV))) return rc;
-  if ((rc = make_tmap_bsc(&tv, v, B, kv_rows, nh * d, ld_kv, kBKV))) return rc;
+  if ((rc = make_tmap_bsc(&tk, k, B, kv_rows, nkv * d, ld_kv, kBKV))) return rc;
+  if ((rc = make_tmap_bsc(&tv, v, B, kv_rows, nkv * d, ld_kv, kBKV))) return rc;
   const float sl2 = scale * kLog2e;
-  if (d == 128) return causal ? launch_fwd<128, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, sl2, st, km, mask_ld)
-                              : launch_fwd<128, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, sl2, st, km, mask_ld);
-  return causal ? launch_fwd<64, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, sl2, st, km, mask_ld)
-                : launch_fwd<64, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, sl2, st, km, mask_ld);
+  const int g = nh / nkv;
+  if (d == 128) return causal ? launch_fwd<128, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
+                              : launch_fwd<128, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
+  return causal ? launch_fwd<64, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
+                : launch_fwd<64, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
 }
 
 static inline int s_pad(int S) { return (S + 63) / 64 * 64; }
@@ -607,8 +624,8 @@ template <int D, bool C>
 static int launch_bwd(const CUtensorMap& tq64, const CUtensorMap& tq128, const CUtensorMap& tk64, const CUtensorMap& tk128,
                       const CUtensorMap& tv64, const CUtensorMap& tv128, const CUtensorMap& tdo64, const CUtensorMap& tdo128,
                       const bf16* dout, const bf16* out, const float* lse, float* delta, float* lse2, const int* seqlens, bf16* dq,
-                      bf16* dk, bf16* dv, long ld_dq, long ld_dkv, int B, int S, int Skv, int nh, long ld_o, float scale,
-                      cudaStream_t st) {
+                      bf16* dk, bf16* dv, long ld_dq, long ld_dkv, int B, int S, int Skv, int nh, int nkv, long ld_o,
+                      float scale, cudaStream_t st) {
   auto k1 = attn_bwd_dkdv_kernel<D, C>;
   auto k2 = attn_bwd_dq_kernel<D, C>;
   static bool once = false;
@@ -620,11 +637,12 @@ static int launch_bwd(const CUtensorMap& tq64, const CUtensorMap& tq128, const C
   if (nh > 384) return DLLM_ERR_SHAPE;   // prep kernel parks nh x 32 floats in (default-limit) shared memory
   attn_bwd_prep_kernel<D><<<static_cast<unsigned>(static_cast<long>(B) * (Sp / 32)), 256, static_cast<size_t>(nh) * 32 * sizeof(float), st>>>(
       dout, out, lse, delta, lse2, B, S, Sp, nh, ld_o);
-  dim3 grid_kv((Skv + 127) / 128, nh, B), grid_q((S + 127) / 128, nh, B);
+  const int group = nh / nkv;
+  dim3 grid_kv((Skv + 127) / 128, nkv, B), grid_q((S + 127) / 128, nh, B);
   k1<<<grid_kv, kAttnThreads, BwdKVSmem<D>::kBytes, st>>>(tq64, tk128, tv128, tdo64, dk, dv, ld_dkv, lse2, delta, seqlens, S, Skv, Sp,
-                                                           nh, scale, scale * kLog2e);
-  k2<<<grid_q, kAttnThreads, BwdQSmem<D>::kBytes, st>>>(tq128, tk64, tv64, tdo128, dq, ld_dq, lse2, delta, seqlens, S, Skv, Sp, nh, scale,
-                                                        scale * kLog2e);
+                                                           nh, group, scale, scale * kLog2e);
+  k2<<<grid_q, kAttnThreads, BwdQSmem<D>::kBytes, st>>>(tq128, tk64, tv64, tdo128, dq, ld_dq, lse2, delta, seqlens, S, Skv, Sp, nh, group,
+                                                        scale, scale * kLog2e);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 
@@ -638,7 +656,16 @@ int attn_bwd(const void* dout, const void* q, const void* k, const void* v, cons
 int attn_bwd_ex(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
                 void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int S, int Skv, int nh,
                 int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, cudaStream_t st) {
+  return attn_bwd_gqa(dout, q, k, v, out, lse, dq, dk, dv, seqlens, workspace, workspace_bytes, B, S, Skv, nh, nh, d, ld_q, ld_kv, ld_o,
+                      ld_dq, ld_dkv, causal, scale, st);
+}
+
+// k, v, dk, dv: [B, Skv, nkv, d], nkv dividing nh.  dK / dV of kv head hk sum the group's q heads hk * group .. hk * group + group - 1.
+int attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                 void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int S, int Skv, int nh,
+                 int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, cudaStream_t st) {
   if (B <= 0 || S <= 0 || Skv <= 0 || nh <= 0) return DLLM_ERR_SHAPE;
+  if (nkv <= 0 || nh % nkv != 0) return DLLM_ERR_SHAPE;
   if (d != 128 && d != 64) return DLLM_ERR_UNSUPPORTED;
   if (S != Skv && (causal || seqlens)) return DLLM_ERR_UNSUPPORTED;
   if (workspace_bytes < attn_bwd_workspace(B, S, nh, d)) return DLLM_ERR_SHAPE;
@@ -649,18 +676,18 @@ int attn_bwd_ex(const void* dout, const void* q, const void* k, const void* v, c
   float* lse2 = delta + static_cast<size_t>(B) * s_pad(S) * nh;
   CUtensorMap tq64, tq128, tk64, tk128, tv64, tv128, tdo64, tdo128;
   int rc;
-  const int C = nh * d;
+  const int C = nh * d, Ckv = nkv * d;
   if ((rc = make_tmap_bsc(&tq64, q, B, S, C, ld_q, 64))) return rc;
   if ((rc = make_tmap_bsc(&tq128, q, B, S, C, ld_q, 128))) return rc;
-  if ((rc = make_tmap_bsc(&tk64, k, B, Skv, C, ld_kv, 64))) return rc;
-  if ((rc = make_tmap_bsc(&tk128, k, B, Skv, C, ld_kv, 128))) return rc;
-  if ((rc = make_tmap_bsc(&tv64, v, B, Skv, C, ld_kv, 64))) return rc;
-  if ((rc = make_tmap_bsc(&tv128, v, B, Skv, C, ld_kv, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tk64, k, B, Skv, Ckv, ld_kv, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tk128, k, B, Skv, Ckv, ld_kv, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tv64, v, B, Skv, Ckv, ld_kv, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tv128, v, B, Skv, Ckv, ld_kv, 128))) return rc;
   if ((rc = make_tmap_bsc(&tdo64, dout, B, S, C, ld_o, 64))) return rc;
   if ((rc = make_tmap_bsc(&tdo128, dout, B, S, C, ld_o, 128))) return rc;
 #define DLLM_BWD(DD, CC)                                                                                                    \
   return launch_bwd<DD, CC>(tq64, tq128, tk64, tk128, tv64, tv128, tdo64, tdo128, (const bf16*)dout, (const bf16*)out, lse, delta, \
-                            lse2, seqlens, (bf16*)dq, (bf16*)dk, (bf16*)dv, ld_dq, ld_dkv, B, S, Skv, nh, ld_o, scale, st)
+                            lse2, seqlens, (bf16*)dq, (bf16*)dk, (bf16*)dv, ld_dq, ld_dkv, B, S, Skv, nh, nkv, ld_o, scale, st)
   if (d == 128) { if (causal) DLLM_BWD(128, true); else DLLM_BWD(128, false); }
   if (causal) DLLM_BWD(64, true); else DLLM_BWD(64, false);
 #undef DLLM_BWD

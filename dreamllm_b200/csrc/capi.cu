@@ -162,6 +162,20 @@ int dllm_attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* 
   return attn_fwd_cache_mask(q, k, v, out, lse, nullptr, kv_mask, mask_ld, B, Sq, Skv, kv_rows, nh, d, ld_q, ld_kv, ld_o, causal, scale,
                              S(stream));
 }
+int dllm_attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
+                      int mask_ld, int B, int Sq, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
+                      float scale, void* stream) {
+  ensure_context(q);
+  return attn_fwd_gqa(q, k, v, out, lse, seqlens, kv_mask, mask_ld, B, Sq, Skv, kv_rows, nh, nkv, d, ld_q, ld_kv, ld_o, causal, scale,
+                      S(stream));
+}
+int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                      void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int Sq, int Skv, int nh,
+                      int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, void* stream) {
+  ensure_context(dout);
+  return attn_bwd_gqa(dout, q, k, v, out, lse, dq, dk, dv, seqlens, workspace, workspace_bytes, B, Sq, Skv, nh, nkv, d, ld_q, ld_kv,
+                      ld_o, ld_dq, ld_dkv, causal, scale, S(stream));
+}
 int dllm_conv3x3_nhwc(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, const void* bias,
                       const void* rowbias, const void* residual, void* stream) {
   ensure_context(x);

@@ -59,28 +59,37 @@ def grad_out_view(params):
     return torch.as_strided(views[0], (rows,) + tuple(views[0].shape[1:]), views[0].stride())
 
 
+def _glued(p, nxt):
+    """True when `p` and the parameter after it (`nxt`, forward order) must share a bucket: the row blocks of one `_fuse_rows` weight, so
+    that the fused wgrad can write all of them at once.  q|k|v are tagged (`_dllm_fused_with_prev`, grouped-query attention makes k/v
+    narrower than q); gate|up and any other same-shaped neighbouring matrices are glued by shape."""
+    return p.dim() == 2 and (getattr(nxt, "_dllm_fused_with_prev", False) or nxt.shape == p.shape)
+
+
+def plan_runs(params, cap_bytes):
+    """Cut `params` (registration = forward order) into runs of at most `cap_bytes`: cut walking BACKWARDS (the order gradients become
+    ready), each run laid out in forward order, never between glued neighbours (`_glued`), always where dtype or device changes.  The one
+    rule both the gradient reducer and `zero.ShardedAdamW` bucket by."""
+    out, run, run_bytes = [], [], 0
+    for p in reversed(params):
+        nb = p.numel() * p.element_size()
+        same = (not run) or (p.dtype == run[0].dtype and p.device == run[0].device)
+        if run and (not same or (not _glued(p, run[-1]) and run_bytes + nb > cap_bytes)):
+            out.append(list(reversed(run)))
+            run, run_bytes = [], 0
+        run.append(p)
+        run_bytes += nb
+    if run:
+        out.append(list(reversed(run)))
+    return out
+
+
 def plan_buckets(params, cap_bytes, late=()):
-    """Cut `params` (registration = forward order) into buckets: runs are cut walking BACKWARDS (the order gradients become ready), each
-    run is laid out in forward order, and a run is never cut between same-shaped neighbouring matrices (the q|k|v and gate|up row blocks
-    of `_fuse_rows` must stay adjacent so the fused wgrad can write all of them at once).  `late` parameters form the last bucket(s)."""
+    """`plan_runs` over the parameters in forward order; `late` parameters form the last bucket(s)."""
     late_ids = {id(p) for p in late}
     main = [p for p in params if id(p) not in late_ids]
     tail = [p for p in params if id(p) in late_ids]
-    out = []
-    for plist in (main, tail):
-        run, run_bytes = [], 0
-        for p in reversed(plist):
-            nb = p.numel() * p.element_size()
-            glued = bool(run) and p.dim() == 2 and run[-1].shape == p.shape
-            same = (not run) or (p.dtype == run[0].dtype and p.device == run[0].device)
-            if run and (not same or (not glued and run_bytes + nb > cap_bytes)):
-                out.append(list(reversed(run)))
-                run, run_bytes = [], 0
-            run.append(p)
-            run_bytes += nb
-        if run:
-            out.append(list(reversed(run)))
-    return out
+    return plan_runs(main, cap_bytes) + plan_runs(tail, cap_bytes)
 
 
 class BucketedGradReducer:

@@ -35,8 +35,9 @@ from .configuration_dreamllm import DreamLLMConfig, deep_instantiate  # noqa: E4
 def _check_supported(config):
     if getattr(config, "pretraining_tp", 1) != 1:
         raise ValueError("pretraining_tp > 1 is out of scope (SURVEY.md §8a row a6)")
-    if getattr(config, "num_key_value_heads", config.num_attention_heads) != config.num_attention_heads:
-        raise ValueError("GQA (num_key_value_heads != num_attention_heads) is not supported on this path")
+    nkv = getattr(config, "num_key_value_heads", config.num_attention_heads)
+    if nkv <= 0 or config.num_attention_heads % nkv != 0:
+        raise ValueError(f"num_attention_heads ({config.num_attention_heads}) must be a multiple of num_key_value_heads ({nkv})")
     if getattr(config, "attention_bias", False):
         raise ValueError("attention_bias=True is not supported")
     if getattr(config, "hidden_act", "silu") != "silu":
@@ -214,6 +215,10 @@ class DreamLLMAttention(nn.Module):
         self.o_proj = nn.Linear(self.num_heads * self.head_dim, self.hidden_size, bias=False)
         self.rotary_emb = RotaryEmbedding(self.head_dim, max_position_embeddings=self.max_position_embeddings,
                                           base=self.rope_theta)
+        # q|k|v are row blocks of one fused weight (`_fuse_rows`): under GQA k/v are narrower than q, so the bucket planners cannot glue
+        # them by equal shape; this tag keeps each one in the same gradient bucket as the block before it (ddp.plan_runs)
+        self.k_proj.weight._dllm_fused_with_prev = True
+        self.v_proj.weight._dllm_fused_with_prev = True
 
 
 DreamLLMFlashAttention2 = DreamLLMAttention  # same kernel either way
@@ -223,6 +228,7 @@ DreamLLMFlashAttention2 = DreamLLMAttention  # same kernel either way
 @dataclass
 class _LayerMeta:
     num_heads: int
+    num_kv_heads: int
     head_dim: int
     inter: int
     eps: float
@@ -232,12 +238,19 @@ class _LayerMeta:
     cos: torch.Tensor
     sin: torch.Tensor
     seqlens: torch.Tensor | None
-    wqkv: torch.Tensor          # fused [3H, H] view
+    wqkv: torch.Tensor          # fused [(nh + 2 nkv) d, H] view
     wgu: torch.Tensor           # fused [2I, H] view
     p_qkv: tuple = ()           # the Parameters behind the fused views / o_proj / down_proj: their `_dllm_grad_view` (set by a gradient
     p_gu: tuple = ()            # reducer or sharded optimizer) lets the wgrad GEMMs write straight into the flat gradient bucket
     p_o: tuple = ()
     p_d: tuple = ()
+
+
+def _split_heads(qkv, B, S, nh, nkv, d):
+    """q [B,S,nh,d], k and v [B,S,nkv,d]: head-slice views of the fused [B*S, (nh + 2 nkv) d] projection buffer.  Sliced after the
+    view so that the token stride stays (nh + 2 nkv) d even when S == 1 (`view` of a slice may give a size-1 dimension any stride)."""
+    x = qkv.view(B, S, nh + 2 * nkv, d)
+    return x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
 
 
 class _DecoderLayerFn(torch.autograd.Function):
@@ -252,15 +265,14 @@ class _DecoderLayerFn(torch.autograd.Function):
     def forward(ctx, x, w_in, wq, wk, wv, wo, w_post, wg, wu, wd, meta: _LayerMeta):
         B, S, H = x.shape
         T = B * S
-        nh, d, I = meta.num_heads, meta.head_dim, meta.inter
+        nh, nkv, d, I = meta.num_heads, meta.num_kv_heads, meta.head_dim, meta.inter
         x2 = x.reshape(T, H)
         if not x2.is_contiguous():
             x2 = x2.contiguous()
         h1, rstd1, _ = ops.rmsnorm_fwd(x2, w_in, meta.eps)
-        qkv = ops.linear(h1, meta.wqkv)                                   # [T, 3H]
-        ops.rope_(qkv, meta.cos, meta.sin, meta.pos, 2 * nh, d)
-        q4 = qkv.view(B, S, 3, nh, d)
-        ao, lse = ops.attn_fwd(q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], causal=True, seqlens=meta.seqlens)
+        qkv = ops.linear(h1, meta.wqkv)                                   # [T, (nh + 2 nkv) d]
+        ops.rope_(qkv, meta.cos, meta.sin, meta.pos, nh + nkv, d)
+        ao, lse = ops.attn_fwd(*_split_heads(qkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
         ao2 = ao.view(T, H)
         o = ops.linear(ao2, wo)
         h2, rstd2, xmid = ops.rmsnorm_fwd(x2, w_post, meta.eps, add=o)    # xmid = x + o
@@ -275,7 +287,7 @@ class _DecoderLayerFn(torch.autograd.Function):
     def backward(ctx, dy):
         x2, w_in, rstd1, h1, qkv, ao2, lse, wo, xmid, w_post, rstd2, h2, gu, act, wd = ctx.saved_tensors
         meta = ctx.meta
-        B, S, nh, d, I = meta.B, meta.S, meta.num_heads, meta.head_dim, meta.inter
+        B, S, nh, nkv, d, I = meta.B, meta.S, meta.num_heads, meta.num_kv_heads, meta.head_dim, meta.inter
         T, H = x2.shape
         need = ctx.needs_input_grad
         dy2 = dy.reshape(T, H)
@@ -297,23 +309,22 @@ class _DecoderLayerFn(torch.autograd.Function):
         dao = ops.linear_dgrad(dxmid, wo)
         dwo = ops.linear_wgrad(dxmid, ao2, out=grad_out_view(meta.p_o)) if need[5] else None
         dqkv = torch.empty_like(qkv)
-        q4 = qkv.view(B, S, 3, nh, d)
-        dq4 = dqkv.view(B, S, 3, nh, d)
-        ops.attn_bwd(dao.view(B, S, H), q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], ao2.view(B, S, H), lse,
-                     dq4[:, :, 0], dq4[:, :, 1], dq4[:, :, 2], causal=True, seqlens=meta.seqlens)
-        ops.rope_(dqkv, meta.cos, meta.sin, meta.pos, 2 * nh, d, backward=True)
+        ops.attn_bwd(dao.view(B, S, H), *_split_heads(qkv, B, S, nh, nkv, d), ao2.view(B, S, H), lse,
+                     *_split_heads(dqkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
+        ops.rope_(dqkv, meta.cos, meta.sin, meta.pos, nh + nkv, d, backward=True)
         dh1 = ops.linear_dgrad(dqkv, meta.wqkv)
         dwq = dwk = dwv = None
         if need[2] or need[3] or need[4]:
             dwqkv = ops.linear_wgrad(dqkv, h1, out=grad_out_view(meta.p_qkv))
-            dwq, dwk, dwv = dwqkv[:H], dwqkv[H:2 * H], dwqkv[2 * H:]
+            dwq, dwk, dwv = dwqkv[:nh * d], dwqkv[nh * d:(nh + nkv) * d], dwqkv[(nh + nkv) * d:]
         dx, dw_in = ops.rmsnorm_bwd(dh1, x2, w_in, rstd1, dres=dxmid, need_dw=need[1])
         return (dx.view(B, S, H) if need[0] else None, dw_in, dwq, dwk, dwv, dwo, dw_post, dwg, dwu, dwd, None)
 
 
 class KVCache:
-    """Preallocated per-layer K/V buffers [B, max_len, nh, d] (token-major, read in place by the attention kernel).  Replaces the
-    reference's per-layer `torch.cat([past, new], dim=2)` tuples (:444-449); opaque to callers, passed as `past_key_values`."""
+    """Preallocated per-layer K/V buffers [B, max_len, num_heads, d] (token-major, read in place by the attention kernel).  Replaces the
+    reference's per-layer `torch.cat([past, new], dim=2)` tuples (:444-449); opaque to callers, passed as `past_key_values`.
+    `num_heads` is the number of KEY/VALUE heads (`num_key_value_heads`: fewer than the query heads under grouped-query attention)."""
 
     def __init__(self, num_layers, batch, max_len, num_heads, head_dim, device, dtype=BF16):
         # zero-filled: the attention kernel reads whole 64-row tiles; rows past the valid length are masked in the softmax (p = 0) but
@@ -399,8 +410,8 @@ class DreamLLMDecoderLayer(nn.Module):
         seqlens = kwargs.get("seqlens")                   # int32 [B] valid lengths (collator / model loop); else derived from the mask
         if seqlens is None and attention_mask is not None:
             seqlens = attention_mask.sum(-1).to(torch.int32).contiguous()
-        meta = _LayerMeta(att.num_heads, att.head_dim, self.mlp.intermediate_size, self.input_layernorm.variance_epsilon,
-                          B, S, pos, cos, sin, seqlens,
+        meta = _LayerMeta(att.num_heads, att.num_key_value_heads, att.head_dim, self.mlp.intermediate_size,
+                          self.input_layernorm.variance_epsilon, B, S, pos, cos, sin, seqlens,
                           _fuse_rows([att.q_proj.weight, att.k_proj.weight, att.v_proj.weight]),
                           _fuse_rows([self.mlp.gate_proj.weight, self.mlp.up_proj.weight]),
                           (att.q_proj.weight, att.k_proj.weight, att.v_proj.weight), (self.mlp.gate_proj.weight, self.mlp.up_proj.weight),
@@ -420,7 +431,7 @@ class DreamLLMDecoderLayer(nn.Module):
         cache, li = past_key_value
         B, S, H = hidden_states.shape
         att, mlp = self.self_attn, self.mlp
-        nh, d, I = att.num_heads, att.head_dim, mlp.intermediate_size
+        nh, nkv, d, I = att.num_heads, att.num_key_value_heads, att.head_dim, mlp.intermediate_size
         start = cache.len
         if start + S > cache.max_len:
             raise ValueError(f"kv-cache overflow: {start} + {S} > {cache.max_len}")
@@ -434,11 +445,11 @@ class DreamLLMDecoderLayer(nn.Module):
         x2 = hidden_states.reshape(B * S, H).contiguous()
         h1, _, _ = ops.rmsnorm_fwd(x2, self.input_layernorm.weight, eps)
         qkv = ops.linear(h1, _fuse_rows([att.q_proj.weight, att.k_proj.weight, att.v_proj.weight]))
-        ops.rope_(qkv, cos, sin, pos, 2 * nh, d)
-        q4 = qkv.view(B, S, 3, nh, d)
-        cache.k[li][:, start:start + S].copy_(q4[:, :, 1])
-        cache.v[li][:, start:start + S].copy_(q4[:, :, 2])
-        ao = ops.attn_fwd_cache(q4[:, :, 0], cache.k[li], cache.v[li], start + S, causal=True, kv_mask=cache.mask)
+        ops.rope_(qkv, cos, sin, pos, nh + nkv, d)
+        q, k, v = _split_heads(qkv, B, S, nh, nkv, d)
+        cache.k[li][:, start:start + S].copy_(k)
+        cache.v[li][:, start:start + S].copy_(v)
+        ao = ops.attn_fwd_cache(q, cache.k[li], cache.v[li], start + S, causal=True, kv_mask=cache.mask)
         o = ops.linear(ao.view(B * S, H), att.o_proj.weight)
         h2, _, xmid = ops.rmsnorm_fwd(x2, self.post_attention_layernorm.weight, eps, add=o)
         gu = ops.linear(h2, _fuse_rows([mlp.gate_proj.weight, mlp.up_proj.weight]))
@@ -738,7 +749,7 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
             B, S, _ = hidden_states.shape
             att = self.layers[0].self_attn
             cache = past_key_values if past_key_values is not None else KVCache(
-                len(self.layers), B, self.config.max_position_embeddings, att.num_heads, att.head_dim, hidden_states.device)
+                len(self.layers), B, self.config.max_position_embeddings, att.num_key_value_heads, att.head_dim, hidden_states.device)
             if attention_mask is not None and attention_mask_has_padding is not False:
                 # padded batch inside the cache (reference :960-962 keeps the 2-D mask for the flash path, whose `_upad_input` drops the
                 # pad keys; positions come from the mask, :1521-1526).  No host sync: the mask is applied whether or not it has zeros.

@@ -316,35 +316,44 @@ def embedding_bwd(ids, dy2d, vocab, out=None, padding_idx=None):
 
 
 # ----------------------------------------------------------------------------------------------- attention
+def _kv_heads(q, k):
+    """Number of kv heads of a [B, S, nkv, d] key view; grouped-query attention when it is a proper divisor of q's heads."""
+    nh, nkv = q.shape[2], k.shape[2]
+    assert nkv > 0 and nh % nkv == 0, f"{nh} query heads are not a multiple of {nkv} kv heads"
+    return nkv
+
+
 def attn_fwd(q, k, v, causal=True, seqlens=None, scale=None):
-    """q,k,v: [B, S, nh, d] views (last two dims dense, token stride shared) — e.g. slices of the fused qkv buffer.
-    returns (out [B,S,nh*d], lse [B,nh,S])."""
+    """q: [B, S, nh, d], k,v: [B, S, nkv, d] views (last two dims dense, token stride shared) — e.g. slices of the fused qkv buffer.
+    nkv divides nh (grouped-query attention; nkv == nh is multi-head).  returns (out [B,S,nh*d], lse [B,nh,S])."""
     _chk_cuda(q, k, v, seqlens)
     B, S, nh, d = q.shape
+    nkv = _kv_heads(q, k)
     for t in (q, k, v):
         assert t.dtype == BF16 and t.stride(3) == 1 and t.stride(2) == d and t.stride(0) == S * t.stride(1)
-    assert q.stride(1) == k.stride(1) == v.stride(1)
+    assert q.stride(1) == k.stride(1) == v.stride(1) and k.shape == v.shape
     out = torch.empty((B, S, nh * d), device=q.device, dtype=BF16)
     lse = torch.empty((B, nh, S), device=q.device, dtype=torch.float32)
     scale = float(d) ** -0.5 if scale is None else float(scale)
-    check(lib().dllm_attn_fwd(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(seqlens), B, S, nh, d, q.stride(1), nh * d,
-                              int(causal), scale, _stream()), "dllm_attn_fwd")
+    check(lib().dllm_attn_fwd_gqa(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(seqlens), 0, 0, B, S, S, S, nh, nkv, d, q.stride(1),
+                                  q.stride(1), nh * d, int(causal), scale, _stream()), "dllm_attn_fwd_gqa")
     LAUNCHES.add(1)
     return out, lse
 
 
 def attn_bwd(dout, q, k, v, out, lse, dq, dk, dv, causal=True, seqlens=None, scale=None):
-    """dq/dk/dv: [B,S,nh,d] views to write into (e.g. slices of a fused dqkv buffer)."""
+    """dq: [B,S,nh,d], dk/dv: [B,S,nkv,d] views to write into (e.g. slices of a fused dqkv buffer)."""
     _chk_cuda(dout, q, k, v, out, lse, dq, dk, dv, seqlens)
     B, S, nh, d = q.shape
+    nkv = _kv_heads(q, k)
     assert dout.is_contiguous() and out.is_contiguous()
-    assert dq.stride(1) == dk.stride(1) == dv.stride(1)
+    assert dq.stride(1) == dk.stride(1) == dv.stride(1) and dk.shape == dv.shape == k.shape
     scale = float(d) ** -0.5 if scale is None else float(scale)
     wsb = lib().dllm_attn_bwd_workspace_bytes(B, S, nh, d)
     ws = torch.empty(max(wsb, 4), device=q.device, dtype=torch.uint8)
-    check(lib().dllm_attn_bwd(_p(dout), _p(q), _p(k), _p(v), _p(out), _p(lse), _p(dq), _p(dk), _p(dv), _p(seqlens), _p(ws),
-                              wsb, B, S, nh, d, q.stride(1), nh * d, dq.stride(1), int(causal), scale, _stream()),
-          "dllm_attn_bwd")
+    check(lib().dllm_attn_bwd_gqa(_p(dout), _p(q), _p(k), _p(v), _p(out), _p(lse), _p(dq), _p(dk), _p(dv), _p(seqlens), _p(ws),
+                                  wsb, B, S, S, nh, nkv, d, q.stride(1), q.stride(1), nh * d, dq.stride(1), dq.stride(1), int(causal),
+                                  scale, _stream()), "dllm_attn_bwd_gqa")
     LAUNCHES.add(3)
     return dq, dk, dv
 
@@ -409,18 +418,8 @@ def zero_rows_(dst2d, idx):
 
 # ----------------------------------------------------------------------------------------------- UNet ops (NHWC bf16)
 def attn_fwd_cross(q, k, v, scale=None):
-    """q [B,Sq,nh,d], k/v [B,Skv,nh,d] (views; k and v share a token stride). Non-causal. returns out [B,Sq,nh*d]."""
-    _chk_cuda(q, k, v)
-    B, Sq, nh, d = q.shape
-    Skv = k.shape[1]
-    assert k.stride(1) == v.stride(1) and q.stride(3) == 1 and k.stride(3) == 1 and q.stride(2) == d and k.stride(2) == d
-    out = torch.empty((B, Sq, nh * d), device=q.device, dtype=BF16)
-    lse = torch.empty((B, nh, Sq), device=q.device, dtype=torch.float32)
-    scale = float(d) ** -0.5 if scale is None else float(scale)
-    check(lib().dllm_attn_fwd_ex(_p(q), _p(k), _p(v), _p(out), _p(lse), 0, B, Sq, Skv, nh, d, q.stride(1), k.stride(1), nh * d, 0,
-                                 scale, _stream()), "dllm_attn_fwd_ex")
-    LAUNCHES.add(1)
-    return out
+    """q [B,Sq,nh,d], k/v [B,Skv,nkv,d] (views; k and v share a token stride; nkv divides nh). Non-causal. returns out [B,Sq,nh*d]."""
+    return attn_fwd_cross_lse(q, k, v, scale)[0]
 
 
 def conv3x3(x_nhwc, w_k, bias=None, rowbias=None, residual=None):
@@ -506,29 +505,30 @@ def geglu_bwd(dout2d, in2d):
 
 
 def attn_bwd_cross(dout, q, k, v, out, lse, dq, dk, dv, scale=None):
-    """q/dq [B,Sq,nh,d]; k,v,dk,dv [B,Skv,nh,d] views (k,v share a token stride; dk,dv share one)."""
+    """q/dq [B,Sq,nh,d]; k,v,dk,dv [B,Skv,nkv,d] views (k,v share a token stride; dk,dv share one; nkv divides nh)."""
     _chk_cuda(dout, q, k, v, out, lse, dq, dk, dv)
     B, Sq, nh, d = q.shape
-    Skv = k.shape[1]
+    Skv, nkv = k.shape[1], _kv_heads(q, k)
     scale = float(d) ** -0.5 if scale is None else float(scale)
     wsb = lib().dllm_attn_bwd_workspace_bytes(B, Sq, nh, d)
     ws = torch.empty(max(wsb, 4), device=q.device, dtype=torch.uint8)
     assert dout.is_contiguous() and out.is_contiguous()
-    check(lib().dllm_attn_bwd_ex(_p(dout), _p(q), _p(k), _p(v), _p(out), _p(lse), _p(dq), _p(dk), _p(dv), 0, _p(ws), wsb, B, Sq, Skv,
-                                 nh, d, q.stride(1), k.stride(1), nh * d, dq.stride(1), dk.stride(1), 0, scale, _stream()),
-          "dllm_attn_bwd_ex")
+    check(lib().dllm_attn_bwd_gqa(_p(dout), _p(q), _p(k), _p(v), _p(out), _p(lse), _p(dq), _p(dk), _p(dv), 0, _p(ws), wsb, B, Sq, Skv,
+                                  nh, nkv, d, q.stride(1), k.stride(1), nh * d, dq.stride(1), dk.stride(1), 0, scale, _stream()),
+          "dllm_attn_bwd_gqa")
     LAUNCHES.add(3)
 
 
 def attn_fwd_cross_lse(q, k, v, scale=None):
     _chk_cuda(q, k, v)
     B, Sq, nh, d = q.shape
-    Skv = k.shape[1]
+    Skv, nkv = k.shape[1], _kv_heads(q, k)
+    assert k.stride(1) == v.stride(1) and q.stride(3) == 1 and k.stride(3) == 1 and q.stride(2) == d and k.stride(2) == d
     out = torch.empty((B, Sq, nh * d), device=q.device, dtype=BF16)
     lse = torch.empty((B, nh, Sq), device=q.device, dtype=torch.float32)
     scale = float(d) ** -0.5 if scale is None else float(scale)
-    check(lib().dllm_attn_fwd_ex(_p(q), _p(k), _p(v), _p(out), _p(lse), 0, B, Sq, Skv, nh, d, q.stride(1), k.stride(1), nh * d, 0,
-                                 scale, _stream()), "dllm_attn_fwd_ex")
+    check(lib().dllm_attn_fwd_gqa(_p(q), _p(k), _p(v), _p(out), _p(lse), 0, 0, 0, B, Sq, Skv, Skv, nh, nkv, d, q.stride(1), k.stride(1),
+                                  nh * d, 0, scale, _stream()), "dllm_attn_fwd_gqa")
     LAUNCHES.add(1)
     return out, lse
 
@@ -744,23 +744,22 @@ def vae_sample(h_nchw_f32, wq, bq, z_f32, scaling):
 
 
 def attn_fwd_cache(q, k_cache, v_cache, kv_len, causal=True, scale=None, kv_mask=None):
-    """q [B,Sq,nh,d] view; k_cache/v_cache [B, max_len, nh, d] (contiguous rows of nh*d), first kv_len rows valid.
+    """q [B,Sq,nh,d] view; k_cache/v_cache [B, max_len, nkv, d] (contiguous rows of nkv*d, nkv divides nh), first kv_len rows valid.
     kv_mask: optional uint8 [B, mask_ld] (0 = padded key position), mask_ld a multiple of 64 covering kv_len."""
     _chk_cuda(q, k_cache, v_cache, kv_mask)
     B, Sq, nh, d = q.shape
-    kv_rows = k_cache.shape[1]
+    kv_rows, nkv = k_cache.shape[1], _kv_heads(q, k_cache)
     assert k_cache.stride(1) == v_cache.stride(1) and k_cache.stride(0) == kv_rows * k_cache.stride(1)
+    assert q.stride(0) == Sq * q.stride(1), "q's batch stride must be Sq token strides (the kernel's TMA map assumes it)"
     out = torch.empty((B, Sq, nh * d), device=q.device, dtype=BF16)
     lse = torch.empty((B, nh, Sq), device=q.device, dtype=torch.float32)
     scale = float(d) ** -0.5 if scale is None else float(scale)
+    mask_ld = 0
     if kv_mask is not None:
         assert kv_mask.dtype == torch.uint8 and kv_mask.dim() == 2 and kv_mask.shape[0] == B and kv_mask.stride(1) == 1
-        check(lib().dllm_attn_fwd_cache_mask(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), _p(kv_mask), kv_mask.stride(0), B, Sq,
-                                             int(kv_len), kv_rows, nh, d, q.stride(1), k_cache.stride(1), nh * d, int(causal), scale,
-                                             _stream()), "dllm_attn_fwd_cache_mask")
-    else:
-        check(lib().dllm_attn_fwd_cache(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), B, Sq, int(kv_len), kv_rows, nh, d, q.stride(1),
-                                        k_cache.stride(1), nh * d, int(causal), scale, _stream()), "dllm_attn_fwd_cache")
+        mask_ld = kv_mask.stride(0)
+    check(lib().dllm_attn_fwd_gqa(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), 0, _p(kv_mask), mask_ld, B, Sq, int(kv_len), kv_rows,
+                                  nh, nkv, d, q.stride(1), k_cache.stride(1), nh * d, int(causal), scale, _stream()), "dllm_attn_fwd_gqa")
     LAUNCHES.add(1)
     return out
 

@@ -29,6 +29,8 @@ import math
 import torch
 import torch.distributed as dist
 
+from .ddp import plan_runs
+
 ALIGN = 128     # elements; every rank's shard starts 256-byte aligned and is a multiple of the kernels' 8-element vectors
 
 
@@ -149,22 +151,9 @@ class ShardedAdamW:
                     raise ValueError("ShardedAdamW steps bf16 parameters (cast the model with .to(torch.bfloat16))")
             grp["params"] = plist
             self.param_groups.append(grp)
-            # buckets = consecutive runs of the group's parameters; runs are cut walking BACKWARDS (the order gradients become ready),
-            # each run is laid out in forward order
-            # never between same-shaped neighbouring matrices: q|k|v and gate|up must stay adjacent for `_fuse_rows`
-            run, run_bytes = [], 0
-            for p in reversed(plist):
-                nb = p.numel() * 2
-                glued = bool(run) and p.dim() == 2 and run[-1].shape == p.shape
-                if run and p.device != run[0].device:
-                    glued = False
-                if run and not glued and (run_bytes + nb > cap or p.device != run[0].device):
-                    self._make_bucket(list(reversed(run)), grp)
-                    run, run_bytes = [], 0
-                run.append(p)
-                run_bytes += nb
-            if run:
-                self._make_bucket(list(reversed(run)), grp)
+            # buckets = consecutive runs of the group's parameters, cut by the gradient reducer's rule (q|k|v and gate|up stay adjacent)
+            for run in plan_runs(plist, cap):
+                self._make_bucket(run, grp)
         self._bucket_of = {}
         for b in self.buckets:
             for p in b.params:

@@ -122,6 +122,18 @@ int dllm_attn_fwd_cache(const void* q, const void* k, const void* v, void* out, 
 int dllm_attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, float* lse, const void* kv_mask, int mask_ld, int B,
                              int Sq, int Skv, int kv_rows, int nh, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale,
                              void* stream);
+/* grouped-query attention (reference repeat_kv, modeling_dreamllm.py:242-252; flash_attn_func takes the narrow K/V directly, :485):
+ * k, v: [B, kv_rows, nkv, d] with nkv dividing nh; q head h attends with kv head h / (nh / nkv).  Covers every case of the forward
+ * entries above: cache rows (kv_rows >= Skv), right-padded `seqlens` (NULL = none) and the cache key mask `kv_mask` (NULL = none).
+ * nkv == nh is multi-head attention, and the entries above are exactly that call.  nkv <= 0 or nh % nkv != 0: invalid shape. */
+int dllm_attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
+                      int mask_ld, int B, int Sq, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
+                      float scale, void* stream);
+/* backward of dllm_attn_fwd_gqa (no kv-cache): dk, dv are [B, Skv, nkv, d] (token stride ld_dkv); the gradient of kv head hk is the sum
+ * over its group of q heads, in a fixed order (bitwise repeatable).  Workspace: dllm_attn_bwd_workspace_bytes(B, Sq, nh, d). */
+int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                      void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int Sq, int Skv, int nh,
+                      int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, void* stream);
 /* ResnetBlock2D / Upsample2D conv: implicit-GEMM 3x3 stride-1 pad-1 on wgmma tensor cores (4-D TMA im2col, zero-fill padding).
  * y = conv(x, w) + bias[c] + rowbias[n, c] (+ residual);  w is [Cout, 3, 3, Cin]. */
 int dllm_conv3x3_nhwc(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, const void* bias,
