@@ -543,6 +543,219 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   store_rows<D>(dqa, dq, ld_dq, b, S, row_t, h * D, c_in, ms);
 }
 
+// ================================================================================================ attention probabilities
+// P = softmax(Q K^T * scale + mask) as a dense bf16 [B, nh, S, Skv] (the eager path's attention weights, reference :357-378), from the
+// forward's lse: one QK^T pass, P = exp2(S * scale log2e - lse log2e), no V and no PV product.  CTA = 128 query rows of one (head, batch),
+// the forward's grid and layout (two warpgroups of 64 rows, K tiles through a two-stage TMA ring).  Row semantics, as the reference's:
+//   * rows with a finite lse: the forward's own statistics;
+//   * right-padded rows (row >= seqlens[b]): the reference masks keys only, so they are a softmax over keys < len.  The forward stores
+//     lse = +inf there, so a CTA holding such rows first runs a statistics pass over K (the forward's online max / sum);
+//   * rows with no visible key (a left-padded prompt position, a length-0 sample): the reference clamps every score to finfo.min, so
+//     the row is uniform, bf16(1 / Skv) in every column.
+// Every element of the output is written exactly once: tiles past the last one with a visible key get no MMA and are written as
+// zeros (or the uniform value).  P tiles are staged in shared memory with each row shifted by its global misalignment, so the rows of
+// an arbitrary width Skv leave as 16-byte stores except for the partial chunk at either end.
+template <int D>
+struct ProbsSmem {
+  static constexpr int NCH = D / 64;
+  static constexpr int kQ = NCH * 16384;         // [NCH][128][128B]
+  static constexpr int kK = NCH * kBKV * 128;    // [NCH][kBKV][128B]
+  static constexpr int kPitch = kBKV + 16;       // staging row (elements): 128 columns + up to 7 of shift, 16-byte multiple
+  static constexpr int oQ = 0, oK = kQ, oP = oK + 2 * kK, oBar = oP + 128 * kPitch * 2;
+  static constexpr int kBytes = oBar + 64 + 1024;
+};
+
+template <int D, bool kCausal>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_probs_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk, const float* __restrict__ lse,
+                  bf16* __restrict__ probs, const int* __restrict__ seqlens, int S, int Skv, int nh, int group, float scale_log2,
+                  const uint8_t* __restrict__ kv_mask, int mask_ld) {
+  using L = ProbsSmem<D>;
+  constexpr int NCH = L::NCH;
+  constexpr int NJ = kBKV / 8;
+  constexpr int P = L::kPitch;
+  const int coff = kCausal ? (Skv - S) : 0;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::oBar);
+  uint64_t* k_full = q_full + 1;                  // [2]
+  bf16* stage = reinterpret_cast<bf16*>(smem + L::oP);
+
+  const int q0 = (kCausal ? (gridDim.x - 1 - blockIdx.x) : blockIdx.x) * 128, h = blockIdx.y, b = blockIdx.z;
+  const int hkv = h / group;
+  const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;
+  const int q_len = seqlens ? kv_len : S;
+  const int kv_end = kCausal ? min(kv_len, q0 + 128 + coff) : kv_len;
+  const int n_kv = kv_end > 0 ? (kv_end + kBKV - 1) / kBKV : 0;   // tiles with a visible key for some row of the CTA
+  const int n_tiles = (Skv + kBKV - 1) / kBKV;
+  const bool stats_pass = min(S, q0 + 128) > q_len;             // the tile holds right-padded rows
+  const int n_items = (stats_pass ? 2 : 1) * n_kv;               // K tiles through the ring: [statistics pass,] write pass
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    mbar_init(&k_full[0], 1);
+    mbar_init(&k_full[1], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  auto load_k = [&](int it) {
+    const int st = it & 1, j = it % n_kv;
+    mbar_arrive_expect_tx(&k_full[st], kBKV * D * 2);
+    for (int c = 0; c < NCH; ++c)
+      tma_load_3d(smem + L::oK + st * L::kK + c * kBKV * 128, &tk, &k_full[st], hkv * D + c * 64, j * kBKV, b);
+  };
+  if (threadIdx.x == 0 && n_items > 0) {
+    mbar_arrive_expect_tx(q_full, 128 * D * 2);
+    for (int c = 0; c < NCH; ++c) tma_load_3d(smem + L::oQ + c * 16384, &tq, q_full, h * D + c * 64, q0, b);
+    load_k(0);
+    if (n_items > 1) load_k(1);
+  }
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c_in = 2 * (t & 3);
+  const int row_t = q0 + wg * 64 + r_in;          // + 8h
+  const uint32_t sQ = smem_u32(smem + L::oQ) + wg * 8192;
+
+  // S = Q K^T of ring item `it` into s, then release its ring stage
+  auto qk = [&](int it, float* s) {
+    const int st = it & 1;
+    mbar_wait(&k_full[st], (it >> 1) & 1, 7);
+    const uint32_t sK = smem_u32(smem + L::oK + st * L::kK);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < D / 16; ++ks) wgmma_ss<kBKV, 0, 0>(s, kmajor_step(kmajor_desc0(sQ), 16384, ks), kmajor_step(kmajor_desc0(sK), kBKV * 128, ks), ks > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncthreads();                                   // both warpgroups are done with ring stage st
+    if (threadIdx.x == 0 && it + 2 < n_items) load_k(it + 2);
+  };
+  // the forward's mask: -inf where the key is past kv_len, padded in kv_mask or (causal) after the query
+  auto mask_tile = [&](float* s, int kv0) {
+    if (!((kCausal && kv0 + kBKV - 1 > q0 + coff) || (kv0 + kBKV > kv_len) || (kv_mask != nullptr))) return;
+#pragma unroll
+    for (int jj = 0; jj < NJ; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int kvi = kv0 + 8 * jj + c_in + e;
+        bool ok = kvi < kv_len;
+        if (ok && kv_mask != nullptr) ok = kv_mask[static_cast<size_t>(b) * mask_ld + kvi] != 0;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          if (!(ok && (!kCausal || kvi <= row_t + 8 * hh + coff))) s[4 * jj + 2 * hh + e] = -INFINITY;
+      }
+  };
+
+  // per row: lse in log2 units, or uniform (no visible key)
+  const float* lse_bh = lse + (static_cast<size_t>(b) * nh + h) * S;
+  float l2[2];
+  bool uni[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int row = row_t + 8 * hh;
+    const float v = row < min(S, q_len) ? lse_bh[row] : INFINITY;
+    uni[hh] = v == INFINITY;
+    l2[hh] = v * kLog2e;
+  }
+  if (n_items > 0) mbar_wait(q_full, 0, 8);
+  int it = 0;
+  if (stats_pass) {
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    for (int j = 0; j < n_kv; ++j, ++it) {
+      float s[kBKV / 2];
+      qk(it, s);
+      mask_tile(s, j * kBKV);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int jj = 0; jj < NJ; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
+        mx = quad_max(mx);
+        const float m_new = fmaxf(m_run[hh], mx * scale_log2);
+        const float alpha = (m_run[hh] == -INFINITY) ? 0.f : exp2f(m_run[hh] - m_new);
+        m_run[hh] = m_new;
+        const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
+        float ls = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < NJ; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) ls += exp2f(s[4 * jj + 2 * hh + e] * scale_log2 - m_use);
+        l_run[hh] = l_run[hh] * alpha + ls;
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float l = quad_sum(l_run[hh]);
+      if (row_t + 8 * hh >= q_len) {
+        uni[hh] = !(l > 0.f);
+        l2[hh] = m_run[hh] + log2f(l);
+      }
+    }
+  }
+
+  const float uval = __frcp_rn(static_cast<float>(Skv));   // the reference's fp32 softmax over Skv equal scores
+  const size_t plane = (static_cast<size_t>(b) * nh + h) * S;
+  for (int j = 0; j < n_tiles; ++j) {
+    const int kv0 = j * kBKV;
+    float s[kBKV / 2];
+    if (j < n_kv) {
+      qk(it++, s);
+      mask_tile(s, kv0);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int jj = 0; jj < NJ; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& x = s[4 * jj + 2 * hh + e];
+            x = uni[hh] ? uval : exp2f(x * scale_log2 - l2[hh]);
+          }
+    } else {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int jj = 0; jj < NJ; ++jj) s[4 * jj + 2 * hh] = s[4 * jj + 2 * hh + 1] = uni[hh] ? uval : 0.f;
+    }
+    // registers -> staging rows, each shifted by m = (its global element index) % 8 so that 16-byte global chunks are 16-byte aligned here
+    named_bar_sync(1 + wg, 128);                       // this warpgroup's previous tile has left the staging rows
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int R = wg * 64 + r_in + 8 * hh;
+      const int m = static_cast<int>(((plane + q0 + R) * Skv + kv0) & 7);
+      bf16* srow = stage + R * P + m;
+#pragma unroll
+      for (int jj = 0; jj < NJ; ++jj) {
+        const float a = s[4 * jj + 2 * hh], c = s[4 * jj + 2 * hh + 1];
+        if ((m & 1) == 0) {
+          *reinterpret_cast<uint32_t*>(srow + 8 * jj + c_in) = pack_bf16(a, c);
+        } else {
+          srow[8 * jj + c_in] = __float2bfloat16_rn(a);
+          srow[8 * jj + c_in + 1] = __float2bfloat16_rn(c);
+        }
+      }
+    }
+    named_bar_sync(1 + wg, 128);
+    // staging -> global: a half-warp per row, lane k of it owns 16-byte chunks k and k + 16 of the row's span
+    const int n = min(kBKV, Skv - kv0), lane16 = t & 15;
+    for (int rr = t >> 4; rr < 64; rr += 8) {
+      const int R = wg * 64 + rr;
+      if (q0 + R >= S) break;
+      const size_t e0 = (plane + q0 + R) * Skv + kv0;
+      const int m = static_cast<int>(e0 & 7);
+      bf16* g = probs + (e0 - m);
+      const bf16* srow = stage + R * P;
+      const int nch = (m + n + 7) >> 3;
+      for (int k = lane16; k < nch; k += 16) {
+        const int lo = 8 * k;
+        if (lo >= m && lo + 8 <= m + n) {
+          *reinterpret_cast<uint4*>(g + lo) = *reinterpret_cast<const uint4*>(srow + lo);
+        } else {
+          for (int c = max(lo, m); c < min(lo + 8, m + n); ++c) g[c] = srow[c];
+        }
+      }
+    }
+  }
+}
+
 // ================================================================================================ host
 template <typename K>
 static int set_smem(K kern, int bytes) {
@@ -615,6 +828,46 @@ int attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* 
                               : launch_fwd<128, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
   return causal ? launch_fwd<64, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
                 : launch_fwd<64, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
+}
+
+template <int D, bool C>
+static int launch_probs(const CUtensorMap& tq, const CUtensorMap& tk, const float* lse, void* probs, const int* seqlens, int B, int S,
+                        int Skv, int nh, int group, float scale_log2, cudaStream_t st, const uint8_t* kv_mask, int mask_ld) {
+  auto kern = attn_probs_kernel<D, C>;
+  static bool once = false;
+  if (!once) {
+    if (set_smem(kern, ProbsSmem<D>::kBytes)) return DLLM_ERR_LAUNCH;
+    once = true;
+  }
+  dim3 grid((S + 127) / 128, nh, B);
+  kern<<<grid, kAttnThreads, ProbsSmem<D>::kBytes, st>>>(tq, tk, lse, static_cast<bf16*>(probs), seqlens, S, Skv, nh, group, scale_log2,
+                                                         kv_mask, mask_ld);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+
+// Attention probabilities [B, nh, S, Skv] bf16 (dense, row-major) of the attention attn_fwd_gqa computed with the same q, k, masks and
+// shapes; `lse` is that call's output.
+int attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, const int* seqlens, const void* kv_mask, int mask_ld,
+                   int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, int causal, float scale,
+                   cudaStream_t st) {
+  if (B <= 0 || S <= 0 || Skv <= 0 || nh <= 0 || kv_rows < Skv) return DLLM_ERR_SHAPE;
+  if (nkv <= 0 || nh % nkv != 0) return DLLM_ERR_SHAPE;
+  if (kv_mask && ((mask_ld & 15) || mask_ld < (Skv + 63) / 64 * 64 || (reinterpret_cast<uintptr_t>(kv_mask) & 15))) return DLLM_ERR_ALIGN;
+  const uint8_t* km = static_cast<const uint8_t*>(kv_mask);
+  if (d != 128 && d != 64) return DLLM_ERR_UNSUPPORTED;
+  if (S != Skv && seqlens) return DLLM_ERR_UNSUPPORTED;
+  if (causal && Skv < S) return DLLM_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(probs) & 15) return DLLM_ERR_ALIGN;
+  CUtensorMap tq, tk;
+  int rc;
+  if ((rc = make_tmap_bsc(&tq, q, B, S, nh * d, ld_q, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tk, k, B, kv_rows, nkv * d, ld_kv, kBKV))) return rc;
+  const float sl2 = scale * kLog2e;
+  const int g = nh / nkv;
+  if (d == 128) return causal ? launch_probs<128, true>(tq, tk, lse, probs, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
+                              : launch_probs<128, false>(tq, tk, lse, probs, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
+  return causal ? launch_probs<64, true>(tq, tk, lse, probs, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
+                : launch_probs<64, false>(tq, tk, lse, probs, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
 }
 
 static inline int s_pad(int S) { return (S + 63) / 64 * 64; }

@@ -169,6 +169,13 @@ int dllm_attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, fl
   return attn_fwd_gqa(q, k, v, out, lse, seqlens, kv_mask, mask_ld, B, Sq, Skv, kv_rows, nh, nkv, d, ld_q, ld_kv, ld_o, causal, scale,
                       S(stream));
 }
+int dllm_attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, const int* seqlens, const void* kv_mask, int mask_ld,
+                        int B, int Sq, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, int causal, float scale,
+                        void* stream) {
+  ensure_context(q);
+  return attn_probs_gqa(q, k, lse, probs, seqlens, kv_mask, mask_ld, B, Sq, Skv, kv_rows, nh, nkv, d, ld_q, ld_kv, causal, scale,
+                        S(stream));
+}
 int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
                       void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int Sq, int Skv, int nh,
                       int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, void* stream) {

@@ -37,6 +37,9 @@ int attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, 
 int attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
                  int mask_ld, int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
                  float scale, cudaStream_t st);
+int attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, const int* seqlens, const void* kv_mask, int mask_ld,
+                   int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, int causal, float scale,
+                   cudaStream_t st);
 size_t groupnorm_workspace(int N, int HW, int G);
 int groupnorm_nhwc(const void* x, const void* w, const void* b, void* y, void* workspace, size_t ws_bytes, int N, int HW, int C,
                    int G, float eps, int silu, cudaStream_t s);

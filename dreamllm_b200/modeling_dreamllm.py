@@ -15,6 +15,8 @@ There is no eager/CPU fallback: modules raise if their tensors are not on a CUDA
 """
 from __future__ import annotations
 
+import functools
+import logging
 import math
 from dataclasses import dataclass
 
@@ -26,6 +28,13 @@ from . import ops
 from .ddp import grad_out_view
 
 BF16 = torch.bfloat16
+logger = logging.getLogger(__name__)
+
+
+@functools.lru_cache(maxsize=None)
+def _warn_once(msg: str):
+    """transformers' `logger.warning_once`."""
+    logger.warning(msg)
 
 
 # ------------------------------------------------------------------------------------------------ config
@@ -244,6 +253,17 @@ class _LayerMeta:
     p_gu: tuple = ()            # reducer or sharded optimizer) lets the wgrad GEMMs write straight into the flat gradient bucket
     p_o: tuple = ()
     p_d: tuple = ()
+    probs: "_AttnProbsSlot | None" = None   # set: also return the attention probabilities (output_attentions)
+
+
+class _AttnProbsSlot:
+    """One layer's attention probabilities, materialised at most once per forward.  Non-reentrant gradient checkpointing runs the layer
+    forward again inside backward with the same kwargs, so the slot passed there still holds the tensor and the recompute reuses it
+    instead of launching the kernel (and allocating B * nh * S * S * 2 bytes) a second time."""
+    __slots__ = ("value",)
+
+    def __init__(self):
+        self.value = None
 
 
 def _split_heads(qkv, B, S, nh, nkv, d):
@@ -259,6 +279,8 @@ class _DecoderLayerFn(torch.autograd.Function):
     fwd: rmsnorm -> qkv GEMM -> rope(in place) -> flash-attn -> o GEMM -> (+residual, rmsnorm fused) -> gate|up GEMM
          -> swiglu -> down GEMM -> +residual
     bwd: the transposed sequence; dgrad = NN GEMM, wgrad = TN GEMM, wgrad skipped for frozen weights.
+    With `meta.probs` set, forward also returns the attention probabilities [B, nh, S, S] (attn_probs kernel after flash-attn, from its
+    lse) as a second, non-differentiable output; y and every gradient are unchanged.
     """
 
     @staticmethod
@@ -273,6 +295,8 @@ class _DecoderLayerFn(torch.autograd.Function):
         qkv = ops.linear(h1, meta.wqkv)                                   # [T, (nh + 2 nkv) d]
         ops.rope_(qkv, meta.cos, meta.sin, meta.pos, nh + nkv, d)
         ao, lse = ops.attn_fwd(*_split_heads(qkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
+        if meta.probs is not None and meta.probs.value is None:
+            meta.probs.value = ops.attn_probs(*_split_heads(qkv, B, S, nh, nkv, d)[:2], lse, causal=True, seqlens=meta.seqlens)
         ao2 = ao.view(T, H)
         o = ops.linear(ao2, wo)
         h2, rstd2, xmid = ops.rmsnorm_fwd(x2, w_post, meta.eps, add=o)    # xmid = x + o
@@ -281,10 +305,13 @@ class _DecoderLayerFn(torch.autograd.Function):
         y = ops.linear(act, wd, residual=xmid)                            # down_proj + residual add fused in the GEMM epilogue
         ctx.save_for_backward(x2, w_in, rstd1, h1, qkv, ao2, lse, wo, xmid, w_post, rstd2, h2, gu, act, wd)
         ctx.meta = meta
-        return y.view(B, S, H)
+        if meta.probs is None:
+            return y.view(B, S, H)
+        ctx.mark_non_differentiable(meta.probs.value)
+        return y.view(B, S, H), meta.probs.value
 
     @staticmethod
-    def backward(ctx, dy):
+    def backward(ctx, dy, *_):
         x2, w_in, rstd1, h1, qkv, ao2, lse, wo, xmid, w_post, rstd2, h2, gu, act, wd = ctx.saved_tensors
         meta = ctx.meta
         B, S, nh, nkv, d, I = meta.B, meta.S, meta.num_heads, meta.num_kv_heads, meta.head_dim, meta.inter
@@ -385,15 +412,19 @@ class DreamLLMDecoderLayer(nn.Module):
     def forward(self, hidden_states, attention_mask=None, position_ids=None, past_key_value=None,
                 output_attentions=False, use_cache=False, **kwargs):
         """Same contract as the reference (:599-654).  `attention_mask` is the 2-D [B, S] padding mask of the
-        flash path (:960-962) or None; right padding as the collator produces (builder_dreamllm.py:467-482)."""
+        flash path (:960-962) or None; right padding as the collator produces (builder_dreamllm.py:467-482).
+
+        `output_attentions=True` returns `(hidden, attn_weights)` (cached path: `(hidden, attn_weights, (cache, layer_idx))`), the
+        reference's order.  attn_weights is the post-softmax bf16 [B, nh, q_len, kv_len] of the eager path (:357-378): masked keys 0,
+        right-padded query rows a softmax over the sample's valid keys, rows with no visible key uniform 1/kv_len.  It costs
+        B * nh * q_len * kv_len * 2 bytes per layer (1.07 GB at B 4, S 2048, 32 heads) and, unlike the reference's, does not require
+        grad: no gradient flows back through it.  hidden and every gradient are bit-identical to `output_attentions=False`."""
         if not hidden_states.is_cuda:
             raise RuntimeError("DreamLLMDecoderLayer (dreamllm_b200) requires CUDA tensors; there is no CPU fallback")
         if hidden_states.dtype != BF16:
             raise ValueError("dreamllm_b200 computes in bf16: cast the model and inputs with .to(torch.bfloat16)")
         if past_key_value is not None:
-            return self._forward_cached(hidden_states, position_ids, past_key_value)
-        if output_attentions:
-            raise ValueError("output_attentions=True needs the materialised eager path, which this build does not have")
+            return self._forward_cached(hidden_states, position_ids, past_key_value, output_attentions)
         B, S, H = hidden_states.shape
         if attention_mask is not None and attention_mask.dim() != 2:
             raise ValueError(
@@ -416,16 +447,21 @@ class DreamLLMDecoderLayer(nn.Module):
                           _fuse_rows([self.mlp.gate_proj.weight, self.mlp.up_proj.weight]),
                           (att.q_proj.weight, att.k_proj.weight, att.v_proj.weight), (self.mlp.gate_proj.weight, self.mlp.up_proj.weight),
                           (att.o_proj.weight,), (self.mlp.down_proj.weight,))
-        y = _DecoderLayerFn.apply(hidden_states, self.input_layernorm.weight, att.q_proj.weight, att.k_proj.weight,
-                                  att.v_proj.weight, att.o_proj.weight, self.post_attention_layernorm.weight,
-                                  self.mlp.gate_proj.weight, self.mlp.up_proj.weight, self.mlp.down_proj.weight, meta)
-        outputs = (y,)
+        if output_attentions:
+            # DreamLLMModel passes its own slot under gradient checkpointing, so that the recompute finds the weights already there
+            slot = kwargs.get("attn_probs_slot")
+            meta.probs = slot if slot is not None else _AttnProbsSlot()
+        outputs = _DecoderLayerFn.apply(hidden_states, self.input_layernorm.weight, att.q_proj.weight, att.k_proj.weight,
+                                        att.v_proj.weight, att.o_proj.weight, self.post_attention_layernorm.weight,
+                                        self.mlp.gate_proj.weight, self.mlp.up_proj.weight, self.mlp.down_proj.weight, meta)
+        if not output_attentions:
+            outputs = (outputs,)
         if use_cache:
             raise ValueError("use_cache=True needs a cache: pass past_key_value=(KVCache, layer_idx) (DreamLLMModel does this)")
         return outputs
 
     @torch.no_grad()
-    def _forward_cached(self, hidden_states, position_ids, past_key_value):
+    def _forward_cached(self, hidden_states, position_ids, past_key_value, output_attentions=False):
         """Inference with a kv-cache (prefill or decode; reference :344-355 / :444-449): new keys/values are appended to
         `cache.k/v[layer]` at rows [cache.len, cache.len + S) and attention runs causally (bottom-right aligned) over all of them."""
         cache, li = past_key_value
@@ -449,11 +485,14 @@ class DreamLLMDecoderLayer(nn.Module):
         q, k, v = _split_heads(qkv, B, S, nh, nkv, d)
         cache.k[li][:, start:start + S].copy_(k)
         cache.v[li][:, start:start + S].copy_(v)
-        ao = ops.attn_fwd_cache(q, cache.k[li], cache.v[li], start + S, causal=True, kv_mask=cache.mask)
+        ao, lse = ops.attn_fwd_cache(q, cache.k[li], cache.v[li], start + S, causal=True, kv_mask=cache.mask, return_lse=True)
         o = ops.linear(ao.view(B * S, H), att.o_proj.weight)
         h2, _, xmid = ops.rmsnorm_fwd(x2, self.post_attention_layernorm.weight, eps, add=o)
         gu = ops.linear(h2, _fuse_rows([mlp.gate_proj.weight, mlp.up_proj.weight]))
         y = ops.linear(ops.swiglu_fwd(gu, I), mlp.down_proj.weight, residual=xmid)
+        if output_attentions:
+            probs = ops.attn_probs(q, cache.k[li], lse, causal=True, kv_len=start + S, kv_mask=cache.mask)
+            return (y.view(B, S, H), probs, (cache, li))
         return (y.view(B, S, H), (cache, li))
 
 
@@ -730,7 +769,23 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
                  attention_mask_has_padding=None, seqlens=None):
         """reference :846-1043.  `attention_mask_has_padding` replaces the `0 in attention_mask` host sync (:962):
         pass False when the collator knows there is no padding (None = decide on the device-free path: keep the
-        mask and let the kernel honour seqlens)."""
+        mask and let the kernel honour seqlens).
+
+        `output_attentions` (None: `config.output_attentions`; forced on by `config.log_attentions`, off by a truthy
+        `config._flash_attn_2_enabled`, :920-932) fills `attentions` with one bf16 [B, nh, q_len, kv_len] per layer, B * nh * q_len *
+        kv_len * 2 bytes each (1.07 GB per layer at B 4, S 2048, 32 heads); see DreamLLMDecoderLayer.forward.  `config.log_attentions` /
+        `config.log_hidden_states` put max |.| of every layer's weights / input (and of the final normed output) into
+        `additional_log_info` under the reference's keys (:988-1032), read back with one device-to-host copy per forward."""
+        cfg = self.config
+        if output_attentions is None:
+            output_attentions = getattr(cfg, "output_attentions", False)
+        log_attentions = getattr(cfg, "log_attentions", False)
+        log_hidden_states = getattr(cfg, "log_hidden_states", False)
+        if log_attentions:
+            output_attentions = True
+        if getattr(cfg, "_flash_attn_2_enabled", False) and output_attentions:
+            output_attentions = False
+            _warn_once("Flash Attention 2.0 is enabled. `output_attentions` is set to `False`.")
         if input_ids is not None and inputs_embeds is not None:
             raise ValueError("You cannot specify both input_ids and inputs_embeds at the same time")
         if input_ids is None and inputs_embeds is None:
@@ -776,26 +831,44 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
                 pos_i32 = torch.arange(Sq, device=hidden_states.device, dtype=torch.int32).repeat(Bq)
             else:
                 pos_i32 = position_ids.to(torch.int32).expand(Bq, Sq).reshape(-1).contiguous()
+        all_attn = () if output_attentions else None
+        logged = []                                       # (key, device scalar) in the reference's order
         for li, layer in enumerate(self.layers):
             if output_hidden_states:
                 all_hidden += (hidden_states,)
+            if log_hidden_states:
+                logged.append((f"hidden_states_layer{li - 1}", hidden_states.detach().abs().max()))
             if cache is not None:
-                hidden_states = layer(hidden_states, position_ids=position_ids, past_key_value=(cache, li), use_cache=True)[0]
+                outs = layer(hidden_states, position_ids=position_ids, past_key_value=(cache, li), use_cache=True,
+                             output_attentions=output_attentions)
             elif self.gradient_checkpointing and self.training and torch.is_grad_enabled():
                 # reference :994-1003.  Saves only the layer input and re-runs the (deterministic) layer forward inside backward: ~2.15 GB
                 # -> 0.27 GB of saved activations per layer at C2 shapes, for one extra forward (+33 % layer FLOPs).  Off by default:
                 # 180 GB holds the whole C2 step without recompute (DESIGN.md §3).
-                hidden_states = torch.utils.checkpoint.checkpoint(layer, hidden_states, attention_mask, position_ids, use_reentrant=False,
-                                                                  seqlens=seqlens, pos_i32=pos_i32)[0]
+                kw = {"output_attentions": True, "attn_probs_slot": _AttnProbsSlot()} if output_attentions else {}
+                outs = torch.utils.checkpoint.checkpoint(layer, hidden_states, attention_mask, position_ids, use_reentrant=False,
+                                                         seqlens=seqlens, pos_i32=pos_i32, **kw)
             else:
-                hidden_states = layer(hidden_states, attention_mask=attention_mask, position_ids=position_ids, seqlens=seqlens,
-                                      pos_i32=pos_i32)[0]
+                outs = layer(hidden_states, attention_mask=attention_mask, position_ids=position_ids, seqlens=seqlens,
+                             pos_i32=pos_i32, output_attentions=output_attentions)
+            hidden_states = outs[0]
+            if output_attentions:
+                all_attn += (outs[1],)
+                if log_attentions:
+                    logged.append((f"attentions_layer{li}", outs[1].abs().max()))
         if cache is not None:
             cache.len += hidden_states.shape[1]
         hidden_states = self.norm(hidden_states)
         if output_hidden_states:
             all_hidden += (hidden_states,)
-        return BaseModelOutputWithPast(last_hidden_state=hidden_states, past_key_values=cache, hidden_states=all_hidden)
+        if log_hidden_states:
+            logged.append((f"hidden_states_layer{len(self.layers) - 1}", hidden_states.detach().abs().max()))
+        info = None
+        if logged:                                        # one device-to-host copy instead of the reference's `.cpu().item()` per layer
+            values = torch.stack([v.float() for _, v in logged]).tolist()
+            info = {k: v for (k, _), v in zip(logged, values)}
+        return BaseModelOutputWithPast(last_hidden_state=hidden_states, past_key_values=cache, hidden_states=all_hidden,
+                                       attentions=all_attn, additional_log_info=info)
 
     # ---- plugins (reference :822-831 `init_plugin_modules` instantiates them from config; here they are attached) ----
     def attach_plugins(self, clip_vision_embedding=None, dream_embedding=None, image_start_id=None, dream_start_id=None):
@@ -832,8 +905,8 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
         if not need_splice:
             return self._forward(input_ids=input_ids, attention_mask=attention_mask, position_ids=position_ids,
                                  past_key_values=past_key_values, inputs_embeds=inputs_embeds, use_cache=use_cache,
-                                 output_hidden_states=output_hidden_states, attention_mask_has_padding=attention_mask_has_padding,
-                                 seqlens=seqlens)
+                                 output_attentions=output_attentions, output_hidden_states=output_hidden_states,
+                                 attention_mask_has_padding=attention_mask_has_padding, seqlens=seqlens)
         from .modeling_plugins import build_splice_plan, splice_embeddings
         if input_ids is None:
             raise ValueError("image / dream splicing needs input_ids")
@@ -856,8 +929,9 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
             image_features = image_features.to(inputs_embeds.dtype)
         inputs_embeds = splice_embeddings(inputs_embeds, image_features, dq, splice_plan)
         return self._forward(attention_mask=attention_mask, position_ids=position_ids, inputs_embeds=inputs_embeds,
-                             past_key_values=past_key_values, use_cache=use_cache, output_hidden_states=output_hidden_states,
-                             attention_mask_has_padding=attention_mask_has_padding, seqlens=seqlens)
+                             past_key_values=past_key_values, use_cache=use_cache, output_attentions=output_attentions,
+                             output_hidden_states=output_hidden_states, attention_mask_has_padding=attention_mask_has_padding,
+                             seqlens=seqlens)
 
     def prepare_dream_queries_with_special_token(self, batch_size: int = 1):
         """reference :1161-1169: embeds of [<dream_start>, dream queries, <dream_end>]."""
@@ -985,7 +1059,7 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
         `stable_diffusion_head` loss (:1441); `sd_kwargs` forwards injected random draws to the head (tests)."""
         out = self.model(input_ids=input_ids, images=images, images_dm=images_dm, attention_mask=attention_mask,
                          position_ids=position_ids, past_key_values=past_key_values, inputs_embeds=inputs_embeds,
-                         use_cache=use_cache, output_hidden_states=output_hidden_states,
+                         use_cache=use_cache, output_attentions=output_attentions, output_hidden_states=output_hidden_states,
                          attention_mask_has_padding=attention_mask_has_padding, input_ids_cpu=input_ids_cpu,
                          splice_plan=splice_plan, seqlens=seqlens)
         hidden = out.last_hidden_state
@@ -1026,8 +1100,9 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
         if loss is not None and sched in ("l1_norm", "l2_norm"):
             loss = loss / (self.loss_weight_lm + self.loss_weight_vm if sched == "l1_norm" else
                            math.sqrt(self.loss_weight_lm ** 2 + self.loss_weight_vm ** 2))
+        info.update(out.additional_log_info or {})                                                   # (:1494-1500)
         return CausalLMOutputWithPast(loss=loss, logits=logits, past_key_values=out.past_key_values, hidden_states=out.hidden_states,
-                                      additional_log_info=info)
+                                      attentions=out.attentions, additional_log_info=info)
 
     def _null_prompt_states(self, Q):
         """reference :1420-1439: the classifier-free-guidance "null prompt" — an LLM pass over

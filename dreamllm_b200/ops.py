@@ -743,9 +743,10 @@ def vae_sample(h_nchw_f32, wq, bq, z_f32, scaling):
     return out
 
 
-def attn_fwd_cache(q, k_cache, v_cache, kv_len, causal=True, scale=None, kv_mask=None):
+def attn_fwd_cache(q, k_cache, v_cache, kv_len, causal=True, scale=None, kv_mask=None, return_lse=False):
     """q [B,Sq,nh,d] view; k_cache/v_cache [B, max_len, nkv, d] (contiguous rows of nkv*d, nkv divides nh), first kv_len rows valid.
-    kv_mask: optional uint8 [B, mask_ld] (0 = padded key position), mask_ld a multiple of 64 covering kv_len."""
+    kv_mask: optional uint8 [B, mask_ld] (0 = padded key position), mask_ld a multiple of 64 covering kv_len.
+    Returns out [B, Sq, nh*d], or (out, lse [B, nh, Sq] fp32) with `return_lse` (what `attn_probs` needs)."""
     _chk_cuda(q, k_cache, v_cache, kv_mask)
     B, Sq, nh, d = q.shape
     kv_rows, nkv = k_cache.shape[1], _kv_heads(q, k_cache)
@@ -760,6 +761,34 @@ def attn_fwd_cache(q, k_cache, v_cache, kv_len, causal=True, scale=None, kv_mask
         mask_ld = kv_mask.stride(0)
     check(lib().dllm_attn_fwd_gqa(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), 0, _p(kv_mask), mask_ld, B, Sq, int(kv_len), kv_rows,
                                   nh, nkv, d, q.stride(1), k_cache.stride(1), nh * d, int(causal), scale, _stream()), "dllm_attn_fwd_gqa")
+    LAUNCHES.add(1)
+    return (out, lse) if return_lse else out
+
+
+def attn_probs(q, k, lse, causal=True, seqlens=None, kv_len=None, kv_mask=None, scale=None, out=None):
+    """Attention probabilities softmax(q k^T * scale + mask) as a contiguous bf16 [B, nh, Sq, Skv] (the reference's eager attention
+    weights, modeling_dreamllm.py:357-378), for the attention `attn_fwd` / `attn_fwd_cache` computed with the same arguments; `lse` is
+    its [B, nh, Sq] output.  q [B, Sq, nh, d] view; k [B, kv_rows, nkv, d] (a slice of the fused qkv buffer or a kv-cache), its first
+    `kv_len` rows (default all) are the keys: Skv = kv_len.  `seqlens` / `kv_mask` as in `attn_fwd` / `attn_fwd_cache`.
+    Masked keys are 0, right-padded query rows (>= seqlens[b]) are a softmax over the sample's valid keys, rows with no visible key are
+    uniform 1/Skv.  Not differentiable.  Costs B * nh * Sq * Skv * 2 bytes of HBM (1.07 GB at B 4, S 2048, 32 heads)."""
+    _chk_cuda(q, k, lse, seqlens, kv_mask, out)
+    B, Sq, nh, d = q.shape
+    kv_rows, nkv = k.shape[1], _kv_heads(q, k)
+    Skv = kv_rows if kv_len is None else int(kv_len)
+    assert q.dtype == k.dtype == BF16 and q.stride(3) == 1 and q.stride(2) == d and k.stride(3) == 1 and k.stride(2) == d
+    assert q.stride(0) == Sq * q.stride(1) and k.stride(0) == kv_rows * k.stride(1)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, nh, Sq)
+    if out is None:
+        out = torch.empty((B, nh, Sq, Skv), device=q.device, dtype=BF16)
+    assert out.dtype == BF16 and out.is_contiguous() and tuple(out.shape) == (B, nh, Sq, Skv)
+    scale = float(d) ** -0.5 if scale is None else float(scale)
+    mask_ld = 0
+    if kv_mask is not None:
+        assert kv_mask.dtype == torch.uint8 and kv_mask.dim() == 2 and kv_mask.shape[0] == B and kv_mask.stride(1) == 1
+        mask_ld = kv_mask.stride(0)
+    check(lib().dllm_attn_probs_gqa(_p(q), _p(k), _p(lse), _p(out), _p(seqlens), _p(kv_mask), mask_ld, B, Sq, Skv, kv_rows, nh, nkv, d,
+                                    q.stride(1), k.stride(1), int(causal), scale, _stream()), "dllm_attn_probs_gqa")
     LAUNCHES.add(1)
     return out
 

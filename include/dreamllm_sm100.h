@@ -129,6 +129,13 @@ int dllm_attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* 
 int dllm_attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
                       int mask_ld, int B, int Sq, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
                       float scale, void* stream);
+/* Attention probabilities of dllm_attn_fwd_gqa (output_attentions, the eager path's weights, modeling_dreamllm.py:357-378): probs is a
+ * dense bf16 [B, nh, Sq, Skv] (row stride Skv, 16-byte aligned base), lse the [B, nh, Sq] output of the dllm_attn_fwd_gqa call with the
+ * same q, k, masks and shapes.  Every element is written: masked keys are 0, a right-padded query row (row >= seqlens[b]) is a softmax
+ * over the sample's keys < seqlens[b], a row with no visible key is uniform 1/Skv.  Same shape / alignment rules as dllm_attn_fwd_gqa. */
+int dllm_attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, const int* seqlens, const void* kv_mask, int mask_ld,
+                        int B, int Sq, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, int causal, float scale,
+                        void* stream);
 /* backward of dllm_attn_fwd_gqa (no kv-cache): dk, dv are [B, Skv, nkv, d] (token stride ld_dkv); the gradient of kv head hk is the sum
  * over its group of q heads, in a fixed order (bitwise repeatable).  Workspace: dllm_attn_bwd_workspace_bytes(B, Sq, nh, d). */
 int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
