@@ -92,6 +92,9 @@ SIGNATURES = {
     "dllm_attn_fwd_gqa": (_i, [_vp] * 7 + [_i, _i, _i, _i, _i, _i, _i, _i, _l, _l, _l, _i, _f, _vp]),
     "dllm_attn_bwd_gqa": (_i, [_vp] * 11 + [_sz, _i, _i, _i, _i, _i, _i, _l, _l, _l, _l, _l, _i, _f, _vp]),
     "dllm_attn_probs_gqa": (_i, [_vp] * 6 + [_i] * 8 + [_l, _l, _i, _f, _vp]),
+    "dllm_attn_fwd_varlen": (_i, [_vp] * 6 + [_i] * 6 + [_l, _l, _l, _i, _f, _vp]),
+    "dllm_attn_bwd_varlen_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dllm_attn_bwd_varlen": (_i, [_vp] * 11 + [_sz] + [_i] * 6 + [_l, _l, _l, _l, _l, _i, _f, _vp]),
     "dllm_conv3x3_nhwc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "dllm_groupnorm_workspace_bytes": (_sz, [_i, _i, _i]),
     "dllm_groupnorm_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _f, _i, _vp]),

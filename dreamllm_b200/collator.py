@@ -15,6 +15,12 @@ derives from `input_ids` with host syncs every step (`torch.where` per sample, `
     num_tokens / num_label_tokens  python ints for throughput / loss bookkeeping (the bench's tokens-per-step)
 
 `DreamLLMForCausalMLM.forward(**batch)` accepts these keys directly (`splice_plan`, `input_ids_cpu`, `attention_mask_has_padding`).
+
+`pack=True` emits the same keys for a packed (unpadded) batch instead: the samples' tokens laid end to end as one row of T =
+sum(len_b) tokens, so that no kernel of the step computes a pad row.  `input_ids` / `labels` / `attention_mask` (all ones) /
+`position_ids` (restarting at 0 in every sample) / `shifted_labels` are [1, T]; `cu_seqlens` int32 [B + 1] says where each sample
+starts, `max_seqlen` (python int) is the longest one; `shifted_labels` is -100 at the last token of every sample, so no label crosses
+a boundary; the splice plan addresses rows of the packed sequence.
 Pure host integer work: no CUDA, no kernels; safe in worker processes.
 """
 from __future__ import annotations
@@ -42,6 +48,7 @@ class DataCollatorForDreamLLMDataset:
     pin_memory: bool = False                # pin the index maps (set in the main process; workers cannot pin)
     pad_to_multiple_of: int | None = None   # optional: round S up (keeps TMA tiles full); reference pads to the batch max only
     extra_keys: tuple = field(default_factory=tuple)
+    pack: bool = False                      # emit one packed [1, T] row + cu_seqlens instead of the right-padded [B, S] rectangle
 
     @classmethod
     def from_model(cls, tokenizer, model, **kw):
@@ -79,6 +86,9 @@ class DataCollatorForDreamLLMDataset:
         right_padded = bool((mask == (torch.arange(mask.shape[1])[None] < seqlens[:, None])).all())
         if not right_padded:
             raise ValueError("attention_mask is not a right-padded prefix mask (the collator pads on the right, builder_dreamllm.py:470-472)")
+        if self.pack:
+            out.update(self._packed(ids, labels, seqlens, images, images_dm))
+            return out
         plan = None
         if images is not None or images_dm is not None:
             plan = build_splice_plan(ids, self.image_start_id if images is not None else -1,
@@ -96,12 +106,53 @@ class DataCollatorForDreamLLMDataset:
                    num_label_tokens=int((shifted != IGNORE_INDEX).sum()))
         return out
 
+    def _packed(self, ids, labels, seqlens, images, images_dm) -> dict:
+        """The packed form of the right-padded `ids` / `labels` [B, S]: their valid prefixes, in batch order, as one [1, T] row."""
+        B, S = ids.shape
+        valid = torch.arange(S)[None] < seqlens[:, None]
+        cu = torch.zeros(B + 1, dtype=torch.int32)
+        cu[1:] = torch.cumsum(seqlens, 0)
+        T = int(cu[-1])
+        if T == 0:
+            raise ValueError("cannot pack a batch without a single token")
+        shifted = torch.full_like(labels, IGNORE_INDEX)
+        shifted[:, :-1] = labels[:, 1:]                    # the pad column after a sample's last token is already -100
+        shifted[torch.arange(B), (seqlens.long() - 1).clamp_(min=0)] = IGNORE_INDEX
+        pids = ids[valid][None]
+        plan = None
+        if images is not None or images_dm is not None:
+            P = self.clip_embed_len if images is not None else 0
+            Q = self.dream_embed_len if images_dm is not None else 0
+            img_id = self.image_start_id if images is not None else -1
+            dream_id = self.dream_start_id if images_dm is not None else -1
+            # build_splice_plan bounds a span by its row's length, which for [1, T] ids is T: bound it by its own sample here
+            room = (seqlens[:, None] - 1 - torch.arange(S)[None])[valid]        # tokens after each position, inside its sample
+            n_img = 0 if images is None else images.shape[0]
+            img_at = (pids[0] == img_id).nonzero()[:n_img, 0]
+            dream_at = (pids[0] == dream_id).nonzero()[:, 0]
+            if bool((room[img_at] < P).any()) or bool((room[dream_at] < Q).any()):
+                raise ValueError("an image / dream-query span runs past the end of its sample (reference assert :1126)")
+            plan = build_splice_plan(pids, img_id, dream_id, P, Q, n_img, None if images_dm is None else images_dm.shape[0], "cpu")
+            if self.pin_memory:
+                plan = plan.pin_memory()
+        pos = (torch.arange(S)[None].expand(B, S))[valid][None]
+        pshift = shifted[valid][None]
+        return dict(input_ids=pids, attention_mask=torch.ones_like(pids), labels=labels[valid][None], position_ids=pos,
+                    input_ids_cpu=pids, splice_plan=plan, attention_mask_has_padding=False, seqlens=seqlens, cu_seqlens=cu,
+                    max_seqlen=int(seqlens.max()), shifted_labels=pshift, num_tokens=T,
+                    num_label_tokens=int((pshift != IGNORE_INDEX).sum()))
+
 
 def to_device(batch: dict, device, non_blocking: bool = True) -> dict:
-    """Move a collated batch to the GPU with async copies only (host-side keys stay on the host)."""
+    """Move a collated batch to the GPU with async copies only (host-side keys stay on the host).  A packed batch keeps `max_seqlen`
+    and `cu_seqlens` on the host: the model validates the boundaries there, without a device read-back, and uploads them itself."""
     out = {}
+    packed = "max_seqlen" in batch
     for k, v in batch.items():
-        if k == "input_ids_cpu" or k in ("num_tokens", "num_label_tokens", "attention_mask_has_padding"):
+        if packed and k == "cu_seqlens":
+            out[k] = v
+            continue
+        if k == "input_ids_cpu" or k in ("num_tokens", "num_label_tokens", "attention_mask_has_padding", "max_seqlen"):
             out[k] = v
         elif isinstance(v, SplicePlan):
             out[k] = v.to(device, non_blocking=non_blocking)

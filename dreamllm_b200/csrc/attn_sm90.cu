@@ -12,6 +12,11 @@
 //   * the ring stage of tile j is refilled with tile j + 2 once both warpgroups have passed the CTA barrier at the end of iteration j.
 // Grouped-query attention: k/v carry nkv = nh / group heads and q head h reads kv head h / group (reference repeat_kv, :242-252).  The
 // forward and dQ kernels only remap the K/V column they load; the dK/dV kernel runs one CTA per kv head and sums the group's q heads.
+// Packed batches (kVarlen instantiations, flash_attn_varlen_func's layout): the B samples lie end to end in one [T, cols] sequence and
+// `seqlens` carries cu_seqlens [B + 1].  The tensor maps are [1, T, cols]; the CTA of (tile i, sample b) loads rows from cu[b] + 128 i, so
+// tiles are aligned to the start of each sample exactly as in the padded layout and the arithmetic of a sample is that of a B = 1 call on
+// it alone.  A tile's tail holds the next sample's rows (or TMA zero fill past T): they are masked as keys and as query rows like the
+// padded layout's pad rows, and never stored; a CTA whose tile starts at or past its sample's length exits before it touches a barrier.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -78,15 +83,16 @@ __device__ __forceinline__ uint64_t kmajor_step(uint64_t d0, uint32_t chunk_byte
 // MN-major operand: K step ks (16 lines) of a tile stored as [MN/64 chunks][K lines][128 B]
 __device__ __forceinline__ uint64_t mnmajor_desc0(uint32_t base, uint32_t chunk_bytes) { return make_smem_desc(base, chunk_bytes, 1024u); }
 __device__ __forceinline__ uint64_t mnmajor_step(uint64_t d0, int ks) { return d0 + ((ks * 2048u) >> 4); }
-// acc [64 rows x D] of warpgroup rows (row0 + r) -> bf16 * mul at dst[(b * S + row) * ld + col0 + col], rows < S only
+// acc [64 rows x D] of warpgroup rows (row_t + 8h) -> bf16 * mul at dst[(base + row) * ld + col0 + col], rows < n_rows only
+// (base, n_rows) = (b * S, S) in the padded layout, (cu[b], the sample's length) in the packed one
 template <int D>
-__device__ __forceinline__ void store_rows(const float* acc, bf16* dst, long ld, int b, int S, int row_t, int col0, int c_in,
+__device__ __forceinline__ void store_rows(const float* acc, bf16* dst, long ld, size_t base, int n_rows, int row_t, int col0, int c_in,
                                            const float* mul) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row_t + 8 * h;
-    if (row >= S) continue;
-    bf16* p = dst + (static_cast<size_t>(b) * S + row) * ld + col0 + c_in;
+    if (row >= n_rows) continue;
+    bf16* p = dst + (base + row) * ld + col0 + c_in;
 #pragma unroll
     for (int j = 0; j < D / 8; ++j)
       *reinterpret_cast<uint32_t*>(p + 8 * j) = pack_bf16(acc[4 * j + 2 * h] * mul[h], acc[4 * j + 2 * h + 1] * mul[h]);
@@ -105,7 +111,7 @@ struct FwdSmem {
   static constexpr int kBytes = oBar + 64 + 1024 /*align slack*/;
 };
 
-template <int D, bool kCausal>
+template <int D, bool kCausal, bool kVarlen>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                 const __grid_constant__ CUtensorMap tv, bf16* __restrict__ out, long ld_o, float* __restrict__ lse,
@@ -124,11 +130,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::oBar);
   uint64_t* kv_full = q_full + 1;                 // [2]
 
+  const int h = blockIdx.y, b = blockIdx.z;
+  // packed: sample b is rows row0 .. row0 + len - 1 of batch entry 0 (S = Skv = T); the grid is sized for the longest sample
+  const int row0 = kVarlen ? seqlens[b] : 0, bz = kVarlen ? 0 : b;
+  const int len = kVarlen ? seqlens[b + 1] - row0 : 0;
+  const int n_qt = kVarlen ? (len + 127) / 128 : gridDim.x;
+  if (kVarlen && static_cast<int>(blockIdx.x) >= n_qt) return;
   // causal: q tile i has i + 1 KV tiles of work; launch the heaviest first so the grid's tail is made of short CTAs (LPT order)
-  const int q0 = (kCausal ? (gridDim.x - 1 - blockIdx.x) : blockIdx.x) * 128, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = (kCausal ? (n_qt - 1 - blockIdx.x) : blockIdx.x) * 128;
   const int hkv = h / group;
-  const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;   // Skv != S only for cross-attention (non-causal)
-  const int q_len = seqlens ? kv_len : S;                    // right-padded self-attention: rows >= len are padding
+  const int kv_len = kVarlen ? len : (seqlens ? min(seqlens[b], Skv) : Skv);   // Skv != S only for cross-attention (non-causal)
+  const int q_len = kVarlen ? len : (seqlens ? kv_len : S);                    // right-padded self-attention: rows >= len are padding
+  const int n_rows = kVarlen ? len : S;                                        // rows of out / lse this sample owns
   const int kv_end = kCausal ? min(kv_len, q0 + 128 + coff) : kv_len;
   const int n_kv = kv_end > 0 ? (kv_end + kBKV - 1) / kBKV : 0;
 
@@ -143,13 +156,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     const int st = j & 1;
     mbar_arrive_expect_tx(&kv_full[st], 2 * kBKV * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + st * L::kKV + c * kBKV * 128, &tk, &kv_full[st], hkv * D + c * 64, j * kBKV, b);
-      tma_load_3d(smem + L::oV + st * L::kKV + c * kBKV * 128, &tv, &kv_full[st], hkv * D + c * 64, j * kBKV, b);
+      tma_load_3d(smem + L::oK + st * L::kKV + c * kBKV * 128, &tk, &kv_full[st], hkv * D + c * 64, row0 + j * kBKV, bz);
+      tma_load_3d(smem + L::oV + st * L::kKV + c * kBKV * 128, &tv, &kv_full[st], hkv * D + c * 64, row0 + j * kBKV, bz);
     }
   };
   if (threadIdx.x == 0 && n_kv > 0) {
     mbar_arrive_expect_tx(q_full, 128 * D * 2);
-    for (int c = 0; c < NCH; ++c) tma_load_3d(smem + L::oQ + c * 16384, &tq, q_full, h * D + c * 64, q0, b);
+    for (int c = 0; c < NCH; ++c) tma_load_3d(smem + L::oQ + c * 16384, &tq, q_full, h * D + c * 64, row0 + q0, bz);
     load_kv(0);
     if (n_kv > 1) load_kv(1);
   }
@@ -237,16 +250,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     const int row = row_t + 8 * hh;
     const bool valid_row = (row < q_len) && l > 0.f;
     inv[hh] = valid_row ? 1.f / l : 0.f;
-    if (row < S && (t & 3) == 0)
-      lse[(static_cast<size_t>(b) * nh + h) * S + row] = valid_row ? (m_run[hh] + log2f(l)) * kLn2 : INFINITY;
+    if (row < n_rows && (t & 3) == 0)
+      lse[(static_cast<size_t>(bz) * nh + h) * S + row0 + row] = valid_row ? (m_run[hh] + log2f(l)) * kLn2 : INFINITY;
   }
-  store_rows<D>(o, out + static_cast<size_t>(0), ld_o, b, S, row_t, h * D, c_in, inv);
+  store_rows<D>(o, out, ld_o, static_cast<size_t>(bz) * S + row0, n_rows, row_t, h * D, c_in, inv);
 }
 
 // ================================================================================================ backward prep
 // delta[b,h,s] = sum_d dO*O ; lse2 = lse*log2(e).
 // Output layout is padded to [B, nh, S_pad] (S_pad = S rounded up to 64, pad entries = 0) so the backward kernels may read a whole
-// 64-row q tile's values without a bound check.
+// 64-row q tile's values without a bound check.  A packed batch runs it as B = 1, S = T with S_pad >= T + 64: the backward kernels read
+// a sample's last q tile up to 63 rows past the sample, i.e. the next sample's (masked) values or, after the last sample, the zero pad.
 // A block owns 32 consecutive tokens of one batch entry and all heads: rows (token, head) are read 16 bytes per thread with four row
 // groups in flight (contiguous: heads are adjacent in memory), the dot products are parked in shared memory as [head][token], and the
 // outputs leave as 128-byte runs along the token axis.
@@ -322,7 +336,7 @@ struct BwdKVSmem {
   static constexpr int kBytes = oBar + 64 + 1024;
 };
 
-template <int D, bool kCausal>
+template <int D, bool kCausal, bool kVarlen>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                      const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, bf16* __restrict__ dk,
@@ -336,8 +350,11 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
   uint64_t* q_full = kv_full + 1;                 // [2]
 
   const int kv0 = blockIdx.x * 128, hk = blockIdx.y, b = blockIdx.z;
-  const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;
-  const int q_len = seqlens ? kv_len : S;
+  const int row0 = kVarlen ? seqlens[b] : 0, bz = kVarlen ? 0 : b;      // packed: see attn_fwd_kernel
+  const int len = kVarlen ? seqlens[b + 1] - row0 : 0;
+  if (kVarlen && kv0 >= len) return;
+  const int kv_len = kVarlen ? len : (seqlens ? min(seqlens[b], Skv) : Skv);
+  const int q_len = kVarlen ? len : (seqlens ? kv_len : S);
   const int i0 = kCausal ? kv0 / 64 : 0;           // first q tile that can see this kv tile
   const int i1 = (kv0 < kv_len) ? (q_len + 63) / 64 : 0;
   const int n_q = max(0, i1 - i0);
@@ -354,15 +371,15 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     const int st = it & 1, g = it / n_q, i = i0 + (it - g * n_q), col = (hk * group + g) * D;
     mbar_arrive_expect_tx(&q_full[st], 2 * 64 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oQ + st * L::kQT + c * 8192, &tq, &q_full[st], col + c * 64, i * 64, b);
-      tma_load_3d(smem + L::oDO + st * L::kQT + c * 8192, &tdo, &q_full[st], col + c * 64, i * 64, b);
+      tma_load_3d(smem + L::oQ + st * L::kQT + c * 8192, &tq, &q_full[st], col + c * 64, row0 + i * 64, bz);
+      tma_load_3d(smem + L::oDO + st * L::kQT + c * 8192, &tdo, &q_full[st], col + c * 64, row0 + i * 64, bz);
     }
   };
   if (threadIdx.x == 0 && n_items > 0) {
     mbar_arrive_expect_tx(kv_full, 2 * 128 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + c * 16384, &tk, kv_full, hk * D + c * 64, kv0, b);
-      tma_load_3d(smem + L::oV + c * 16384, &tv, kv_full, hk * D + c * 64, kv0, b);
+      tma_load_3d(smem + L::oK + c * 16384, &tk, kv_full, hk * D + c * 64, row0 + kv0, bz);
+      tma_load_3d(smem + L::oV + c * 16384, &tv, kv_full, hk * D + c * 64, row0 + kv0, bz);
     }
     load_q(0);
     if (n_items > 1) load_q(1);
@@ -378,8 +395,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
   if (n_items > 0) mbar_wait(kv_full, 0, 3);
   for (int it = 0; it < n_items; ++it) {
     const int st = it & 1, g = it / n_q, i = i0 + (it - g * n_q);
-    const float* lse_bh = lse2 + (static_cast<size_t>(b) * nh + hk * group + g) * Sp;
-    const float* del_bh = delta + (static_cast<size_t>(b) * nh + hk * group + g) * Sp;
+    const float* lse_bh = lse2 + (static_cast<size_t>(bz) * nh + hk * group + g) * Sp + row0;
+    const float* del_bh = delta + (static_cast<size_t>(bz) * nh + hk * group + g) * Sp + row0;
     mbar_wait(&q_full[st], (it >> 1) & 1, 4);
     const uint32_t sQ = smem_u32(smem + L::oQ + st * L::kQT), sDO = smem_u32(smem + L::oDO + st * L::kQT);
     float sa[32], dpa[32];
@@ -422,8 +439,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     if (threadIdx.x == 0 && it + 2 < n_items) load_q(it + 2);
   }
   const float ms[2] = {scale, scale}, one[2] = {1.f, 1.f};
-  store_rows<D>(dka, dk, ld_dkv, b, Skv, row_t, hk * D, c_in, ms);
-  store_rows<D>(dva, dv, ld_dkv, b, Skv, row_t, hk * D, c_in, one);
+  const size_t base = static_cast<size_t>(bz) * Skv + row0;
+  store_rows<D>(dka, dk, ld_dkv, base, kVarlen ? len : Skv, row_t, hk * D, c_in, ms);
+  store_rows<D>(dva, dv, ld_dkv, base, kVarlen ? len : Skv, row_t, hk * D, c_in, one);
 }
 
 // ================================================================================================ backward: dQ
@@ -438,7 +456,7 @@ struct BwdQSmem {
   static constexpr int kBytes = oBar + 64 + 1024;
 };
 
-template <int D, bool kCausal>
+template <int D, bool kCausal, bool kVarlen>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                    const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, bf16* __restrict__ dq,
@@ -451,10 +469,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::oBar);
   uint64_t* kv_full = q_full + 1;                 // [2]
 
-  const int q0 = (kCausal ? (gridDim.x - 1 - blockIdx.x) : blockIdx.x) * 128, h = blockIdx.y, b = blockIdx.z;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int row0 = kVarlen ? seqlens[b] : 0, bz = kVarlen ? 0 : b;      // packed: see attn_fwd_kernel
+  const int len = kVarlen ? seqlens[b + 1] - row0 : 0;
+  const int n_qt = kVarlen ? (len + 127) / 128 : gridDim.x;
+  if (kVarlen && static_cast<int>(blockIdx.x) >= n_qt) return;
+  const int q0 = (kCausal ? (n_qt - 1 - blockIdx.x) : blockIdx.x) * 128;
   const int hkv = h / group;
-  const int kv_len = seqlens ? min(seqlens[b], Skv) : Skv;
-  const int q_len = seqlens ? kv_len : S;
+  const int kv_len = kVarlen ? len : (seqlens ? min(seqlens[b], Skv) : Skv);
+  const int q_len = kVarlen ? len : (seqlens ? kv_len : S);
   const int kv_end = (q0 < q_len) ? (kCausal ? min(kv_len, q0 + 128) : kv_len) : 0;
   const int n_kv = kv_end > 0 ? (kv_end + 63) / 64 : 0;
 
@@ -469,15 +492,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
     const int st = j & 1;
     mbar_arrive_expect_tx(&kv_full[st], 2 * 64 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oK + st * L::kKT + c * 8192, &tk, &kv_full[st], hkv * D + c * 64, j * 64, b);
-      tma_load_3d(smem + L::oV + st * L::kKT + c * 8192, &tv, &kv_full[st], hkv * D + c * 64, j * 64, b);
+      tma_load_3d(smem + L::oK + st * L::kKT + c * 8192, &tk, &kv_full[st], hkv * D + c * 64, row0 + j * 64, bz);
+      tma_load_3d(smem + L::oV + st * L::kKT + c * 8192, &tv, &kv_full[st], hkv * D + c * 64, row0 + j * 64, bz);
     }
   };
   if (threadIdx.x == 0 && n_kv > 0) {
     mbar_arrive_expect_tx(q_full, 2 * 128 * D * 2);
     for (int c = 0; c < NCH; ++c) {
-      tma_load_3d(smem + L::oQ + c * 16384, &tq, q_full, h * D + c * 64, q0, b);
-      tma_load_3d(smem + L::oDO + c * 16384, &tdo, q_full, h * D + c * 64, q0, b);
+      tma_load_3d(smem + L::oQ + c * 16384, &tq, q_full, h * D + c * 64, row0 + q0, bz);
+      tma_load_3d(smem + L::oDO + c * 16384, &tdo, q_full, h * D + c * 64, row0 + q0, bz);
     }
     load_kv(0);
     if (n_kv > 1) load_kv(1);
@@ -487,12 +510,12 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c_in = 2 * (t & 3);
   const int row_t = q0 + wg * 64 + r_in;
   const uint32_t sQ = smem_u32(smem + L::oQ) + wg * 8192, sDO = smem_u32(smem + L::oDO) + wg * 8192;
-  const float* lse_bh = lse2 + (static_cast<size_t>(b) * nh + h) * Sp;
-  const float* del_bh = delta + (static_cast<size_t>(b) * nh + h) * Sp;
+  const float* lse_bh = lse2 + (static_cast<size_t>(bz) * nh + h) * Sp;
+  const float* del_bh = delta + (static_cast<size_t>(bz) * nh + h) * Sp;
   float l2[2], dl[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    const int row = min(row_t + 8 * hh, Sp - 1);
+    const int row = min(row0 + row_t + 8 * hh, Sp - 1);
     l2[hh] = lse_bh[row];
     dl[hh] = del_bh[row];
   }
@@ -540,7 +563,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant
     if (threadIdx.x == 0 && j + 2 < n_kv) load_kv(j + 2);
   }
   const float ms[2] = {scale, scale};
-  store_rows<D>(dqa, dq, ld_dq, b, S, row_t, h * D, c_in, ms);
+  store_rows<D>(dqa, dq, ld_dq, static_cast<size_t>(bz) * S + row0, kVarlen ? len : S, row_t, h * D, c_in, ms);
 }
 
 // ================================================================================================ attention probabilities
@@ -762,17 +785,18 @@ static int set_smem(K kern, int bytes) {
   return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 
-template <int D, bool C>
+// grid_rows: rows the grid's tile axis covers (S; packed: the longest sample, with S = Skv = T and seqlens = cu_seqlens)
+template <int D, bool C, bool V = false>
 static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, void* out, long ld_o, float* lse,
                       const int* seqlens, int B, int S, int Skv, int nh, int group, float scale_log2, cudaStream_t st,
-                      const uint8_t* kv_mask, int mask_ld) {
-  auto kern = attn_fwd_kernel<D, C>;
+                      const uint8_t* kv_mask, int mask_ld, int grid_rows) {
+  auto kern = attn_fwd_kernel<D, C, V>;
   static bool once = false;
   if (!once) {
     if (set_smem(kern, FwdSmem<D>::kBytes)) return DLLM_ERR_LAUNCH;
     once = true;
   }
-  dim3 grid((S + 127) / 128, nh, B);
+  dim3 grid((grid_rows + 127) / 128, nh, B);
   kern<<<grid, kAttnThreads, FwdSmem<D>::kBytes, st>>>(tq, tk, tv, static_cast<bf16*>(out), ld_o, lse, seqlens, S, Skv, nh, group,
                                                        scale_log2, kv_mask, mask_ld);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
@@ -824,10 +848,33 @@ int attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* 
   if ((rc = make_tmap_bsc(&tv, v, B, kv_rows, nkv * d, ld_kv, kBKV))) return rc;
   const float sl2 = scale * kLog2e;
   const int g = nh / nkv;
-  if (d == 128) return causal ? launch_fwd<128, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
-                              : launch_fwd<128, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
-  return causal ? launch_fwd<64, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld)
-                : launch_fwd<64, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld);
+  if (d == 128) return causal ? launch_fwd<128, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld, S)
+                              : launch_fwd<128, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld, S);
+  return causal ? launch_fwd<64, true>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld, S)
+                : launch_fwd<64, false>(tq, tk, tv, out, ld_o, lse, seqlens, B, S, Skv, nh, g, sl2, st, km, mask_ld, S);
+}
+
+// Packed batch: q [T, nh, d], k / v [T, nkv, d], out [T, nh * d], lse [nh, T]; cu_seqlens int32 [B + 1] on the device, non-decreasing
+// with cu[0] = 0 and cu[B] = T (trusted, as is max_seqlen >= every length: the Python layer checks them on the host).  Self-attention
+// inside each sample; sample b's rows equal attn_fwd_gqa on that sample alone, bit for bit.
+int attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* cu_seqlens, int B, int T,
+                    int max_seqlen, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, cudaStream_t st) {
+  if (B <= 0 || T <= 0 || nh <= 0 || max_seqlen <= 0 || max_seqlen > T || !cu_seqlens) return DLLM_ERR_SHAPE;
+  if (nkv <= 0 || nh % nkv != 0) return DLLM_ERR_SHAPE;
+  if (d != 128 && d != 64) return DLLM_ERR_UNSUPPORTED;
+  if ((reinterpret_cast<uintptr_t>(out) & 15) || (ld_o & 7)) return DLLM_ERR_ALIGN;
+  CUtensorMap tq, tk, tv;
+  int rc;
+  if ((rc = make_tmap_bsc(&tq, q, 1, T, nh * d, ld_q, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tk, k, 1, T, nkv * d, ld_kv, kBKV))) return rc;
+  if ((rc = make_tmap_bsc(&tv, v, 1, T, nkv * d, ld_kv, kBKV))) return rc;
+  const float sl2 = scale * kLog2e;
+  const int g = nh / nkv;
+#define DLLM_FWDV(DD, CC) \
+  return launch_fwd<DD, CC, true>(tq, tk, tv, out, ld_o, lse, cu_seqlens, B, T, T, nh, g, sl2, st, nullptr, 0, max_seqlen)
+  if (d == 128) { if (causal) DLLM_FWDV(128, true); else DLLM_FWDV(128, false); }
+  if (causal) DLLM_FWDV(64, true); else DLLM_FWDV(64, false);
+#undef DLLM_FWDV
 }
 
 template <int D, bool C>
@@ -873,25 +920,29 @@ int attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, 
 static inline int s_pad(int S) { return (S + 63) / 64 * 64; }
 size_t attn_bwd_workspace(int B, int S, int nh, int) { return static_cast<size_t>(B) * s_pad(S) * nh * 2 * sizeof(float); }
 
-template <int D, bool C>
+// packed: one [nh, T_pad] plane each for delta and lse2, T_pad = T rounded up to 64 plus one 64-row tile of zeros (see the prep kernel)
+static inline int t_pad(int T) { return s_pad(T) + 64; }
+size_t attn_bwd_varlen_workspace(int T, int nh, int) { return static_cast<size_t>(t_pad(T)) * nh * 2 * sizeof(float); }
+
+// packed (V): S = Skv = T, seqlens = cu_seqlens and max_seqlen sizes the tile axis of both grids; Sp = row pitch of delta / lse2
+template <int D, bool C, bool V = false>
 static int launch_bwd(const CUtensorMap& tq64, const CUtensorMap& tq128, const CUtensorMap& tk64, const CUtensorMap& tk128,
                       const CUtensorMap& tv64, const CUtensorMap& tv128, const CUtensorMap& tdo64, const CUtensorMap& tdo128,
                       const bf16* dout, const bf16* out, const float* lse, float* delta, float* lse2, const int* seqlens, bf16* dq,
                       bf16* dk, bf16* dv, long ld_dq, long ld_dkv, int B, int S, int Skv, int nh, int nkv, long ld_o,
-                      float scale, cudaStream_t st) {
-  auto k1 = attn_bwd_dkdv_kernel<D, C>;
-  auto k2 = attn_bwd_dq_kernel<D, C>;
+                      float scale, cudaStream_t st, int max_seqlen, int Sp) {
+  auto k1 = attn_bwd_dkdv_kernel<D, C, V>;
+  auto k2 = attn_bwd_dq_kernel<D, C, V>;
   static bool once = false;
   if (!once) {
     if (set_smem(k1, BwdKVSmem<D>::kBytes) || set_smem(k2, BwdQSmem<D>::kBytes)) return DLLM_ERR_LAUNCH;
     once = true;
   }
-  const int Sp = s_pad(S);
   if (nh > 384) return DLLM_ERR_SHAPE;   // prep kernel parks nh x 32 floats in (default-limit) shared memory
-  attn_bwd_prep_kernel<D><<<static_cast<unsigned>(static_cast<long>(B) * (Sp / 32)), 256, static_cast<size_t>(nh) * 32 * sizeof(float), st>>>(
-      dout, out, lse, delta, lse2, B, S, Sp, nh, ld_o);
+  attn_bwd_prep_kernel<D><<<static_cast<unsigned>(static_cast<long>(V ? 1 : B) * (Sp / 32)), 256, static_cast<size_t>(nh) * 32 * sizeof(float), st>>>(
+      dout, out, lse, delta, lse2, V ? 1 : B, S, Sp, nh, ld_o);
   const int group = nh / nkv;
-  dim3 grid_kv((Skv + 127) / 128, nkv, B), grid_q((S + 127) / 128, nh, B);
+  dim3 grid_kv(((V ? max_seqlen : Skv) + 127) / 128, nkv, B), grid_q(((V ? max_seqlen : S) + 127) / 128, nh, B);
   k1<<<grid_kv, kAttnThreads, BwdKVSmem<D>::kBytes, st>>>(tq64, tk128, tv128, tdo64, dk, dv, ld_dkv, lse2, delta, seqlens, S, Skv, Sp,
                                                            nh, group, scale, scale * kLog2e);
   k2<<<grid_q, kAttnThreads, BwdQSmem<D>::kBytes, st>>>(tq128, tk64, tv64, tdo128, dq, ld_dq, lse2, delta, seqlens, S, Skv, Sp, nh, group,
@@ -940,10 +991,46 @@ int attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, 
   if ((rc = make_tmap_bsc(&tdo128, dout, B, S, C, ld_o, 128))) return rc;
 #define DLLM_BWD(DD, CC)                                                                                                    \
   return launch_bwd<DD, CC>(tq64, tq128, tk64, tk128, tv64, tv128, tdo64, tdo128, (const bf16*)dout, (const bf16*)out, lse, delta, \
-                            lse2, seqlens, (bf16*)dq, (bf16*)dk, (bf16*)dv, ld_dq, ld_dkv, B, S, Skv, nh, nkv, ld_o, scale, st)
+                            lse2, seqlens, (bf16*)dq, (bf16*)dk, (bf16*)dv, ld_dq, ld_dkv, B, S, Skv, nh, nkv, ld_o, scale, st, 0, s_pad(S))
   if (d == 128) { if (causal) DLLM_BWD(128, true); else DLLM_BWD(128, false); }
   if (causal) DLLM_BWD(64, true); else DLLM_BWD(64, false);
 #undef DLLM_BWD
+}
+
+// Backward of attn_fwd_varlen: dq [T, nh, d], dk / dv [T, nkv, d]; every row is written exactly once, by its own sample's CTAs, and
+// sample b's rows equal attn_bwd_gqa on that sample alone, bit for bit.  Workspace: attn_bwd_varlen_workspace(T, nh, d).
+int attn_bwd_varlen(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                    void* dk, void* dv, const int* cu_seqlens, void* workspace, size_t workspace_bytes, int B, int T, int max_seqlen,
+                    int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale,
+                    cudaStream_t st) {
+  if (B <= 0 || T <= 0 || nh <= 0 || max_seqlen <= 0 || max_seqlen > T || !cu_seqlens) return DLLM_ERR_SHAPE;
+  if (nkv <= 0 || nh % nkv != 0) return DLLM_ERR_SHAPE;
+  if (d != 128 && d != 64) return DLLM_ERR_UNSUPPORTED;
+  if (workspace_bytes < attn_bwd_varlen_workspace(T, nh, d)) return DLLM_ERR_SHAPE;
+  if ((reinterpret_cast<uintptr_t>(dq) & 15) || (reinterpret_cast<uintptr_t>(dk) & 15) || (reinterpret_cast<uintptr_t>(dv) & 15) ||
+      (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(dout) & 15) || (ld_dq & 7) || (ld_dkv & 7) || (ld_o & 7))
+    return DLLM_ERR_ALIGN;
+  const int Tp = t_pad(T);
+  float* delta = static_cast<float*>(workspace);
+  float* lse2 = delta + static_cast<size_t>(Tp) * nh;
+  CUtensorMap tq64, tq128, tk64, tk128, tv64, tv128, tdo64, tdo128;
+  int rc;
+  const int C = nh * d, Ckv = nkv * d;
+  if ((rc = make_tmap_bsc(&tq64, q, 1, T, C, ld_q, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tq128, q, 1, T, C, ld_q, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tk64, k, 1, T, Ckv, ld_kv, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tk128, k, 1, T, Ckv, ld_kv, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tv64, v, 1, T, Ckv, ld_kv, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tv128, v, 1, T, Ckv, ld_kv, 128))) return rc;
+  if ((rc = make_tmap_bsc(&tdo64, dout, 1, T, C, ld_o, 64))) return rc;
+  if ((rc = make_tmap_bsc(&tdo128, dout, 1, T, C, ld_o, 128))) return rc;
+#define DLLM_BWDV(DD, CC)                                                                                                          \
+  return launch_bwd<DD, CC, true>(tq64, tq128, tk64, tk128, tv64, tv128, tdo64, tdo128, (const bf16*)dout, (const bf16*)out, lse, \
+                                  delta, lse2, cu_seqlens, (bf16*)dq, (bf16*)dk, (bf16*)dv, ld_dq, ld_dkv, B, T, T, nh, nkv, ld_o, \
+                                  scale, st, max_seqlen, Tp)
+  if (d == 128) { if (causal) DLLM_BWDV(128, true); else DLLM_BWDV(128, false); }
+  if (causal) DLLM_BWDV(64, true); else DLLM_BWDV(64, false);
+#undef DLLM_BWDV
 }
 
 }  // namespace dllm

@@ -183,6 +183,20 @@ int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void
   return attn_bwd_gqa(dout, q, k, v, out, lse, dq, dk, dv, seqlens, workspace, workspace_bytes, B, Sq, Skv, nh, nkv, d, ld_q, ld_kv,
                       ld_o, ld_dq, ld_dkv, causal, scale, S(stream));
 }
+int dllm_attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* cu_seqlens, int B, int T,
+                         int max_seqlen, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, void* stream) {
+  ensure_context(q);
+  return attn_fwd_varlen(q, k, v, out, lse, cu_seqlens, B, T, max_seqlen, nh, nkv, d, ld_q, ld_kv, ld_o, causal, scale, S(stream));
+}
+size_t dllm_attn_bwd_varlen_workspace_bytes(int T, int nh, int d) { return attn_bwd_varlen_workspace(T, nh, d); }
+int dllm_attn_bwd_varlen(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                         void* dk, void* dv, const int* cu_seqlens, void* workspace, size_t workspace_bytes, int B, int T, int max_seqlen,
+                         int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale,
+                         void* stream) {
+  ensure_context(dout);
+  return attn_bwd_varlen(dout, q, k, v, out, lse, dq, dk, dv, cu_seqlens, workspace, workspace_bytes, B, T, max_seqlen, nh, nkv, d, ld_q,
+                         ld_kv, ld_o, ld_dq, ld_dkv, causal, scale, S(stream));
+}
 int dllm_conv3x3_nhwc(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, const void* bias,
                       const void* rowbias, const void* residual, void* stream) {
   ensure_context(x);

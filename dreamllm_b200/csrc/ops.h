@@ -37,6 +37,8 @@ int attn_fwd_cache_mask(const void* q, const void* k, const void* v, void* out, 
 int attn_fwd_gqa(const void* q, const void* k, const void* v, void* out, float* lse, const int* seqlens, const void* kv_mask,
                  int mask_ld, int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal,
                  float scale, cudaStream_t st);
+int attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* cu_seqlens, int B, int T,
+                    int max_seqlen, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, cudaStream_t st);
 int attn_probs_gqa(const void* q, const void* k, const float* lse, void* probs, const int* seqlens, const void* kv_mask, int mask_ld,
                    int B, int S, int Skv, int kv_rows, int nh, int nkv, int d, long ld_q, long ld_kv, int causal, float scale,
                    cudaStream_t st);
@@ -67,6 +69,11 @@ int attn_bwd_ex(const void* dout, const void* q, const void* k, const void* v, c
 int attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
                  void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int S, int Skv, int nh,
                  int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, cudaStream_t s);
+size_t attn_bwd_varlen_workspace(int T, int nh, int d);
+int attn_bwd_varlen(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                    void* dk, void* dv, const int* cu_seqlens, void* workspace, size_t workspace_bytes, int B, int T, int max_seqlen,
+                    int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale,
+                    cudaStream_t s);
 int groupnorm_bwd_nhwc(const void* dy, const void* x, const void* w, const void* b, const float* stats, const void* dres, void* dx,
                        void* workspace, size_t ws_bytes, int N, int HW, int C, int G, int silu, cudaStream_t s);
 int groupnorm_stats(const void* x, float* stats, void* workspace, size_t ws_bytes, int N, int HW, int C, int G, float eps, cudaStream_t s);

@@ -254,6 +254,8 @@ class _LayerMeta:
     p_o: tuple = ()
     p_d: tuple = ()
     probs: "_AttnProbsSlot | None" = None   # set: also return the attention probabilities (output_attentions)
+    cu_seqlens: torch.Tensor | None = None  # set: x is a packed batch [1, T, H]; int32 [n_samples + 1] sample boundaries (device)
+    max_seqlen: int = 0                     # packed: the longest sample (host int, sizes the attention grid)
 
 
 class _AttnProbsSlot:
@@ -273,6 +275,32 @@ def _split_heads(qkv, B, S, nh, nkv, d):
     return x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
 
 
+def _packed_batch(cu_seqlens, max_seqlen, T, device):
+    """(cu_seqlens as device int32, max_seqlen as int) of a packed batch of T tokens.  A host `cu_seqlens` (what the collator emits and
+    `to_device` leaves on the host) is validated here and uploaded with one small async copy; a device tensor is trusted as the kernels
+    trust it, because checking it would cost a device-to-host sync every step."""
+    if not torch.is_tensor(cu_seqlens) or cu_seqlens.dim() != 1 or cu_seqlens.numel() < 2:
+        raise ValueError("cu_seqlens must be a 1-D tensor [n_samples + 1]")
+    if cu_seqlens.is_cuda:
+        return cu_seqlens.to(device=device, dtype=torch.int32).contiguous(), int(max_seqlen)
+    cu = cu_seqlens.to(torch.int64)
+    lens = cu[1:] - cu[:-1]
+    if int(cu[0]) != 0 or int(cu[-1]) != T:
+        raise ValueError(f"cu_seqlens must run from 0 to the number of packed tokens ({T}), got {int(cu[0])} .. {int(cu[-1])}")
+    if bool((lens < 0).any()):
+        raise ValueError("cu_seqlens must be non-decreasing")
+    longest = int(lens.max())
+    if int(max_seqlen) < longest or int(max_seqlen) > T:
+        raise ValueError(f"max_seqlen ({max_seqlen}) must bound every sample length (longest {longest}) and not exceed {T}")
+    return cu_seqlens.to(torch.int32).to(device, non_blocking=True), int(max_seqlen)
+
+
+def _packed_positions(cu_seqlens, T):
+    """int32 [T] RoPE positions restarting at 0 in every sample, built on the device (`output_size` keeps it free of a host sync)."""
+    starts = torch.repeat_interleave(cu_seqlens[:-1], cu_seqlens[1:] - cu_seqlens[:-1], output_size=T)
+    return torch.arange(T, device=cu_seqlens.device, dtype=torch.int32) - starts
+
+
 class _DecoderLayerFn(torch.autograd.Function):
     """One DreamLLMDecoderLayer forward/backward (reference :599-654) as a fixed kernel sequence:
 
@@ -281,6 +309,8 @@ class _DecoderLayerFn(torch.autograd.Function):
     bwd: the transposed sequence; dgrad = NN GEMM, wgrad = TN GEMM, wgrad skipped for frozen weights.
     With `meta.probs` set, forward also returns the attention probabilities [B, nh, S, S] (attn_probs kernel after flash-attn, from its
     lse) as a second, non-differentiable output; y and every gradient are unchanged.
+    With `meta.cu_seqlens` set, x is a packed batch [1, T, H] and only the two attention calls differ (variable-length kernels): every
+    other kernel of the sequence is token-major and takes its RoPE position per token.
     """
 
     @staticmethod
@@ -294,7 +324,10 @@ class _DecoderLayerFn(torch.autograd.Function):
         h1, rstd1, _ = ops.rmsnorm_fwd(x2, w_in, meta.eps)
         qkv = ops.linear(h1, meta.wqkv)                                   # [T, (nh + 2 nkv) d]
         ops.rope_(qkv, meta.cos, meta.sin, meta.pos, nh + nkv, d)
-        ao, lse = ops.attn_fwd(*_split_heads(qkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
+        if meta.cu_seqlens is not None:
+            ao, lse = ops.attn_fwd_varlen(*(t[0] for t in _split_heads(qkv, 1, T, nh, nkv, d)), meta.cu_seqlens, meta.max_seqlen, causal=True)
+        else:
+            ao, lse = ops.attn_fwd(*_split_heads(qkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
         if meta.probs is not None and meta.probs.value is None:
             meta.probs.value = ops.attn_probs(*_split_heads(qkv, B, S, nh, nkv, d)[:2], lse, causal=True, seqlens=meta.seqlens)
         ao2 = ao.view(T, H)
@@ -336,8 +369,12 @@ class _DecoderLayerFn(torch.autograd.Function):
         dao = ops.linear_dgrad(dxmid, wo)
         dwo = ops.linear_wgrad(dxmid, ao2, out=grad_out_view(meta.p_o)) if need[5] else None
         dqkv = torch.empty_like(qkv)
-        ops.attn_bwd(dao.view(B, S, H), *_split_heads(qkv, B, S, nh, nkv, d), ao2.view(B, S, H), lse,
-                     *_split_heads(dqkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
+        if meta.cu_seqlens is not None:
+            ops.attn_bwd_varlen(dao, *(t[0] for t in _split_heads(qkv, 1, T, nh, nkv, d)), ao2, lse,
+                                *(t[0] for t in _split_heads(dqkv, 1, T, nh, nkv, d)), meta.cu_seqlens, meta.max_seqlen, causal=True)
+        else:
+            ops.attn_bwd(dao.view(B, S, H), *_split_heads(qkv, B, S, nh, nkv, d), ao2.view(B, S, H), lse,
+                         *_split_heads(dqkv, B, S, nh, nkv, d), causal=True, seqlens=meta.seqlens)
         ops.rope_(dqkv, meta.cos, meta.sin, meta.pos, nh + nkv, d, backward=True)
         dh1 = ops.linear_dgrad(dqkv, meta.wqkv)
         dwq = dwk = dwv = None
@@ -418,11 +455,25 @@ class DreamLLMDecoderLayer(nn.Module):
         reference's order.  attn_weights is the post-softmax bf16 [B, nh, q_len, kv_len] of the eager path (:357-378): masked keys 0,
         right-padded query rows a softmax over the sample's valid keys, rows with no visible key uniform 1/kv_len.  It costs
         B * nh * q_len * kv_len * 2 bytes per layer (1.07 GB at B 4, S 2048, 32 heads) and, unlike the reference's, does not require
-        grad: no gradient flows back through it.  hidden and every gradient are bit-identical to `output_attentions=False`."""
+        grad: no gradient flows back through it.  hidden and every gradient are bit-identical to `output_attentions=False`.
+
+        `cu_seqlens=` (int32 [n_samples + 1]) together with `max_seqlen=` (host int) makes `hidden_states` a packed batch [1, T, H]: the samples' tokens end
+        to end, each attending only to itself, positions restarting at 0 in every sample unless `position_ids` says otherwise.  It
+        computes what the right-padded batch computes with the pad rows deleted.  Training only: no kv-cache, no `output_attentions`."""
         if not hidden_states.is_cuda:
             raise RuntimeError("DreamLLMDecoderLayer (dreamllm_b200) requires CUDA tensors; there is no CPU fallback")
         if hidden_states.dtype != BF16:
             raise ValueError("dreamllm_b200 computes in bf16: cast the model and inputs with .to(torch.bfloat16)")
+        max_seqlen = kwargs.get("max_seqlen")
+        cu_seqlens = kwargs.get("cu_seqlens") if max_seqlen is not None else None    # a packed batch is announced by both
+        if cu_seqlens is not None:
+            if past_key_value is not None or use_cache:
+                raise ValueError("a packed batch (cu_seqlens) cannot be combined with a kv-cache (past_key_value / use_cache)")
+            if output_attentions:
+                raise ValueError("output_attentions is not available for a packed batch (cu_seqlens): the weights are a dense [B, nh, S, S]")
+            if hidden_states.shape[0] != 1:
+                raise ValueError(f"a packed batch is [1, T, hidden], got {tuple(hidden_states.shape)}")
+            cu_seqlens, max_seqlen = _packed_batch(cu_seqlens, max_seqlen, hidden_states.shape[1], hidden_states.device)
         if past_key_value is not None:
             return self._forward_cached(hidden_states, position_ids, past_key_value, output_attentions)
         B, S, H = hidden_states.shape
@@ -433,13 +484,17 @@ class DreamLLMDecoderLayer(nn.Module):
         dev = hidden_states.device
         pos = kwargs.get("pos_i32")                       # [B*S] int32, built once per forward by DreamLLMModel._forward
         if pos is None:
-            if position_ids is None:
+            if position_ids is None and cu_seqlens is not None:
+                pos = _packed_positions(cu_seqlens, S)
+            elif position_ids is None:
                 pos = torch.arange(S, device=dev, dtype=torch.int32).repeat(B)
             else:
                 pos = position_ids.to(torch.int32).expand(B, S).reshape(-1).contiguous()
         cos, sin = att.rotary_emb.tables(max(S, att.max_position_embeddings), dev)
         seqlens = kwargs.get("seqlens")                   # int32 [B] valid lengths (collator / model loop); else derived from the mask
-        if seqlens is None and attention_mask is not None:
+        if cu_seqlens is not None:
+            seqlens = None                                # a packed batch has no pad rows
+        elif seqlens is None and attention_mask is not None:
             seqlens = attention_mask.sum(-1).to(torch.int32).contiguous()
         meta = _LayerMeta(att.num_heads, att.num_key_value_heads, att.head_dim, self.mlp.intermediate_size,
                           self.input_layernorm.variance_epsilon, B, S, pos, cos, sin, seqlens,
@@ -447,6 +502,8 @@ class DreamLLMDecoderLayer(nn.Module):
                           _fuse_rows([self.mlp.gate_proj.weight, self.mlp.up_proj.weight]),
                           (att.q_proj.weight, att.k_proj.weight, att.v_proj.weight), (self.mlp.gate_proj.weight, self.mlp.up_proj.weight),
                           (att.o_proj.weight,), (self.mlp.down_proj.weight,))
+        if cu_seqlens is not None:
+            meta.cu_seqlens, meta.max_seqlen = cu_seqlens, max_seqlen
         if output_attentions:
             # DreamLLMModel passes its own slot under gradient checkpointing, so that the recompute finds the weights already there
             slot = kwargs.get("attn_probs_slot")
@@ -766,7 +823,7 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
 
     def _forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None, inputs_embeds=None,
                  use_cache=None, output_attentions=None, output_hidden_states=None, return_dict=None,
-                 attention_mask_has_padding=None, seqlens=None):
+                 attention_mask_has_padding=None, seqlens=None, cu_seqlens=None, max_seqlen=None):
         """reference :846-1043.  `attention_mask_has_padding` replaces the `0 in attention_mask` host sync (:962):
         pass False when the collator knows there is no padding (None = decide on the device-free path: keep the
         mask and let the kernel honour seqlens).
@@ -775,7 +832,11 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
         `config._flash_attn_2_enabled`, :920-932) fills `attentions` with one bf16 [B, nh, q_len, kv_len] per layer, B * nh * q_len *
         kv_len * 2 bytes each (1.07 GB per layer at B 4, S 2048, 32 heads); see DreamLLMDecoderLayer.forward.  `config.log_attentions` /
         `config.log_hidden_states` put max |.| of every layer's weights / input (and of the final normed output) into
-        `additional_log_info` under the reference's keys (:988-1032), read back with one device-to-host copy per forward."""
+        `additional_log_info` under the reference's keys (:988-1032), read back with one device-to-host copy per forward.
+
+        `cu_seqlens` with `max_seqlen`: a packed batch, `input_ids` / `inputs_embeds` [1, T] (see DreamLLMDecoderLayer.forward and
+        collator.py `pack=True`).  Pass `cu_seqlens` as the collator's host tensor to have it validated without a device read-back.
+        `cu_seqlens` without `max_seqlen` is what the collator adds to a right-padded batch for bookkeeping: it changes nothing."""
         cfg = self.config
         if output_attentions is None:
             output_attentions = getattr(cfg, "output_attentions", False)
@@ -792,6 +853,21 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
             raise ValueError("You have to specify either input_ids or inputs_embeds")
         if inputs_embeds is None:
             inputs_embeds = _EmbeddingFn.apply(input_ids, self.embed_tokens.weight, self.embed_tokens.padding_idx)
+        if max_seqlen is None:
+            cu_seqlens = None
+        if cu_seqlens is not None:
+            if use_cache or past_key_values is not None:
+                raise ValueError("a packed batch (cu_seqlens) cannot be combined with a kv-cache (past_key_values / use_cache)")
+            if output_attentions:
+                raise ValueError("output_attentions / log_attentions are not available for a packed batch (cu_seqlens): the weights "
+                                 "are a dense [B, nh, S, S]")
+            if inputs_embeds.shape[0] != 1:
+                raise ValueError(f"a packed batch is one row of T tokens, got batch {inputs_embeds.shape[0]}")
+            if attention_mask_has_padding or (attention_mask_has_padding is None and attention_mask is not None
+                                              and not bool(attention_mask.all())):
+                raise ValueError("a packed batch has no padding: attention_mask must be all ones (or None)")
+            cu_seqlens, max_seqlen = _packed_batch(cu_seqlens, max_seqlen, inputs_embeds.shape[1], inputs_embeds.device)
+            attention_mask_has_padding = False
         if attention_mask_has_padding is False:
             attention_mask = None
             seqlens = None
@@ -827,10 +903,13 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
             elif seqlens is not None:
                 seqlens = seqlens.to(device=hidden_states.device, dtype=torch.int32).contiguous()
             Bq, Sq = hidden_states.shape[:2]
-            if position_ids is None:
+            if position_ids is None and cu_seqlens is not None:
+                pos_i32 = _packed_positions(cu_seqlens, Sq)
+            elif position_ids is None:
                 pos_i32 = torch.arange(Sq, device=hidden_states.device, dtype=torch.int32).repeat(Bq)
             else:
                 pos_i32 = position_ids.to(torch.int32).expand(Bq, Sq).reshape(-1).contiguous()
+        packed = {} if cu_seqlens is None else {"cu_seqlens": cu_seqlens, "max_seqlen": max_seqlen}
         all_attn = () if output_attentions else None
         logged = []                                       # (key, device scalar) in the reference's order
         for li, layer in enumerate(self.layers):
@@ -847,10 +926,10 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
                 # 180 GB holds the whole C2 step without recompute (DESIGN.md §3).
                 kw = {"output_attentions": True, "attn_probs_slot": _AttnProbsSlot()} if output_attentions else {}
                 outs = torch.utils.checkpoint.checkpoint(layer, hidden_states, attention_mask, position_ids, use_reentrant=False,
-                                                         seqlens=seqlens, pos_i32=pos_i32, **kw)
+                                                         seqlens=seqlens, pos_i32=pos_i32, **packed, **kw)
             else:
                 outs = layer(hidden_states, attention_mask=attention_mask, position_ids=position_ids, seqlens=seqlens,
-                             pos_i32=pos_i32, output_attentions=output_attentions)
+                             pos_i32=pos_i32, output_attentions=output_attentions, **packed)
             hidden_states = outs[0]
             if output_attentions:
                 all_attn += (outs[1],)
@@ -887,10 +966,13 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
 
     def forward(self, input_ids=None, images=None, images_dm=None, attention_mask=None, position_ids=None,
                 past_key_values=None, inputs_embeds=None, use_cache=None, output_attentions=None, output_hidden_states=None,
-                return_dict=None, attention_mask_has_padding=None, input_ids_cpu=None, splice_plan=None, seqlens=None):
+                return_dict=None, attention_mask_has_padding=None, input_ids_cpu=None, splice_plan=None, seqlens=None,
+                cu_seqlens=None, max_seqlen=None):
         """reference :1045-1158: embed_tokens -> dream-query splice -> CLIP features -> image splice -> `_forward`.
         `input_ids_cpu` (the collator's host copy) lets the index maps be built without a device->host sync;
-        `splice_plan` lets the caller pass prebuilt maps (SURVEY §8f row 3)."""
+        `splice_plan` lets the caller pass prebuilt maps (SURVEY §8f row 3).  Packed batches (`cu_seqlens`, `_forward`): the plan is built
+        over the [1, T] ids, where batch-major order is the packed order; that an image or dream-query span stays inside its own sample is
+        checked by the collator, which knows the boundaries."""
         # reference :1059-1064: with `freeze_embed_tokens` + newly added special tokens, only the last `num_added_tokens` rows may
         # move — the original rows are restored from the backup every forward (projects/dreamllm/train.py:149-155 sets both attributes)
         backup = getattr(self, "embed_tokens_backup", None)
@@ -906,7 +988,8 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
             return self._forward(input_ids=input_ids, attention_mask=attention_mask, position_ids=position_ids,
                                  past_key_values=past_key_values, inputs_embeds=inputs_embeds, use_cache=use_cache,
                                  output_attentions=output_attentions, output_hidden_states=output_hidden_states,
-                                 attention_mask_has_padding=attention_mask_has_padding, seqlens=seqlens)
+                                 attention_mask_has_padding=attention_mask_has_padding, seqlens=seqlens, cu_seqlens=cu_seqlens,
+                                 max_seqlen=max_seqlen)
         from .modeling_plugins import build_splice_plan, splice_embeddings
         if input_ids is None:
             raise ValueError("image / dream splicing needs input_ids")
@@ -931,7 +1014,7 @@ class DreamLLMModel(DreamLLMPreTrainedModel):
         return self._forward(attention_mask=attention_mask, position_ids=position_ids, inputs_embeds=inputs_embeds,
                              past_key_values=past_key_values, use_cache=use_cache, output_attentions=output_attentions,
                              output_hidden_states=output_hidden_states, attention_mask_has_padding=attention_mask_has_padding,
-                             seqlens=seqlens)
+                             seqlens=seqlens, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
 
     def prepare_dream_queries_with_special_token(self, batch_size: int = 1):
         """reference :1161-1169: embeds of [<dream_start>, dream queries, <dream_end>]."""
@@ -1052,16 +1135,18 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
     def forward(self, input_ids=None, images=None, images_dm=None, attention_mask=None, position_ids=None,
                 past_key_values=None, inputs_embeds=None, labels=None, use_cache=None, output_attentions=None,
                 output_hidden_states=None, return_dict=None, attention_mask_has_padding=None, input_ids_cpu=None,
-                splice_plan=None, sd_kwargs=None, seqlens=None, shifted_labels=None, **kwargs):
+                splice_plan=None, sd_kwargs=None, seqlens=None, shifted_labels=None, cu_seqlens=None, max_seqlen=None, **kwargs):
         """reference :1353-1509.  `seqlens` / `shifted_labels` / `splice_plan` / `input_ids_cpu` are the collator's precomputed maps
         (dreamllm_b200/collator.py, SURVEY §8f row 3); without them they are derived here as the reference does.  Comprehension path: images -> CLIP -> splice -> LM loss.  Creation path: dream-query conditioning
         gather (:1401-1418, also returned in `additional_log_info["dream_conditioning"]`) -> optional null-prompt pass (:1420-1439) ->
-        `stable_diffusion_head` loss (:1441); `sd_kwargs` forwards injected random draws to the head (tests)."""
+        `stable_diffusion_head` loss (:1441); `sd_kwargs` forwards injected random draws to the head (tests).
+        `cu_seqlens` / `max_seqlen`: a packed batch (`input_ids` / `labels` [1, T], DreamLLMModel._forward); labels derived here get -100
+        at the last token of every sample, so that no sample is asked to predict the next one's first token."""
         out = self.model(input_ids=input_ids, images=images, images_dm=images_dm, attention_mask=attention_mask,
                          position_ids=position_ids, past_key_values=past_key_values, inputs_embeds=inputs_embeds,
                          use_cache=use_cache, output_attentions=output_attentions, output_hidden_states=output_hidden_states,
                          attention_mask_has_padding=attention_mask_has_padding, input_ids_cpu=input_ids_cpu,
-                         splice_plan=splice_plan, seqlens=seqlens)
+                         splice_plan=splice_plan, seqlens=seqlens, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
         hidden = out.last_hidden_state
         B, S, H = hidden.shape
         h2 = hidden.reshape(B * S, H)
@@ -1074,6 +1159,10 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
             else:
                 shifted = torch.full_like(labels, -100)
                 shifted[:, :-1] = labels[:, 1:]
+                if cu_seqlens is not None and max_seqlen is not None:
+                    # (cu[1:] - 1) % T: an empty first sample wraps to the last token, which is -100 already
+                    ends = (cu_seqlens[1:].to(shifted.device, non_blocking=True).long() - 1) % shifted.shape[1]
+                    shifted[0].index_fill_(0, ends, -100)
             lm_loss = _LMHeadLossFn.apply(h2, self.lm_head.weight, shifted.reshape(-1).contiguous())
             loss = lm_loss * self.loss_weight_lm
         elif kwargs.get("last_token_logits_only", False):

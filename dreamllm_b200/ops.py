@@ -358,6 +358,49 @@ def attn_bwd(dout, q, k, v, out, lse, dq, dk, dv, causal=True, seqlens=None, sca
     return dq, dk, dv
 
 
+def _chk_varlen(q, k, v, cu_seqlens):
+    T, nh, d = q.shape
+    nkv = k.shape[1]
+    assert nkv > 0 and nh % nkv == 0, f"{nh} query heads are not a multiple of {nkv} kv heads"
+    for t in (q, k, v):
+        assert t.dtype == BF16 and t.stride(2) == 1 and t.stride(1) == d
+    assert q.stride(0) == k.stride(0) == v.stride(0) and k.shape == v.shape == (T, nkv, d)
+    assert cu_seqlens.dtype == torch.int32 and cu_seqlens.dim() == 1 and cu_seqlens.is_contiguous() and cu_seqlens.numel() >= 2
+    return cu_seqlens.numel() - 1, T, nh, nkv, d
+
+
+def attn_fwd_varlen(q, k, v, cu_seqlens, max_seqlen, causal=True, scale=None):
+    """Packed batch (B samples end to end, T tokens in all).  q: [T, nh, d], k,v: [T, nkv, d] views (last dim dense, token stride
+    shared) — e.g. slices of the fused qkv buffer; cu_seqlens int32 [B + 1] on the device (cu[0] = 0, cu[B] = T, non-decreasing) and
+    max_seqlen a host int >= every length: neither is read back here, the caller validates them on its host copy.
+    returns (out [T, nh*d], lse [nh, T])."""
+    _chk_cuda(q, k, v, cu_seqlens)
+    B, T, nh, nkv, d = _chk_varlen(q, k, v, cu_seqlens)
+    out = torch.empty((T, nh * d), device=q.device, dtype=BF16)
+    lse = torch.empty((nh, T), device=q.device, dtype=torch.float32)
+    scale = float(d) ** -0.5 if scale is None else float(scale)
+    check(lib().dllm_attn_fwd_varlen(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(cu_seqlens), B, T, int(max_seqlen), nh, nkv, d,
+                                     q.stride(0), q.stride(0), nh * d, int(causal), scale, _stream()), "dllm_attn_fwd_varlen")
+    LAUNCHES.add(1)
+    return out, lse
+
+
+def attn_bwd_varlen(dout, q, k, v, out, lse, dq, dk, dv, cu_seqlens, max_seqlen, causal=True, scale=None):
+    """dq: [T, nh, d], dk/dv: [T, nkv, d] views to write into (e.g. slices of a fused dqkv buffer)."""
+    _chk_cuda(dout, q, k, v, out, lse, dq, dk, dv, cu_seqlens)
+    B, T, nh, nkv, d = _chk_varlen(q, k, v, cu_seqlens)
+    assert dout.is_contiguous() and out.is_contiguous()
+    assert dq.stride(0) == dk.stride(0) == dv.stride(0) and dk.shape == dv.shape == k.shape
+    scale = float(d) ** -0.5 if scale is None else float(scale)
+    wsb = lib().dllm_attn_bwd_varlen_workspace_bytes(T, nh, d)
+    ws = torch.empty(wsb, device=q.device, dtype=torch.uint8)
+    check(lib().dllm_attn_bwd_varlen(_p(dout), _p(q), _p(k), _p(v), _p(out), _p(lse), _p(dq), _p(dk), _p(dv), _p(cu_seqlens), _p(ws),
+                                     wsb, B, T, int(max_seqlen), nh, nkv, d, q.stride(0), q.stride(0), nh * d, dq.stride(0),
+                                     dq.stride(0), int(causal), scale, _stream()), "dllm_attn_bwd_varlen")
+    LAUNCHES.add(3)
+    return dq, dk, dv
+
+
 # ----------------------------------------------------------------------------------------------- CLIP / splice helpers
 def layernorm_fwd(x2d, weight, bias, eps):
     _chk_cuda(x2d, weight, bias)

@@ -141,6 +141,23 @@ int dllm_attn_probs_gqa(const void* q, const void* k, const float* lse, void* pr
 int dllm_attn_bwd_gqa(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
                       void* dk, void* dv, const int* seqlens, void* workspace, size_t workspace_bytes, int B, int Sq, int Skv, int nh,
                       int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale, void* stream);
+/* Packed (unpadded) batches, the layout of flash_attn_varlen_func (reference modeling_dreamllm.py:532, :553-583): B samples laid end to
+ * end as T = sum(len_b) tokens.  q: [T, nh, d], k, v: [T, nkv, d] views (token strides ld_q / ld_kv), out: [T, nh*d] (ld_o), lse:
+ * [nh, T] fp32.  cu_seqlens: device int32 [B + 1], non-decreasing, cu[0] = 0, cu[B] = T; sample b owns rows cu[b] .. cu[b+1] - 1 and
+ * attends only to itself (zero-length samples are legal).  max_seqlen (host) bounds every length and sizes the grid.  cu_seqlens and
+ * max_seqlen are trusted: validate them on the host.  Every row of out / lse is written exactly once, and the rows of sample b equal,
+ * bit for bit, dllm_attn_fwd_gqa on that sample alone (B = 1, Sq = Skv = len_b).  NULL cu_seqlens, max_seqlen <= 0 or > T: invalid
+ * shape. */
+int dllm_attn_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int* cu_seqlens, int B, int T,
+                         int max_seqlen, int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, int causal, float scale, void* stream);
+/* backward of dllm_attn_fwd_varlen: dq [T, nh, d] (ld_dq), dk, dv [T, nkv, d] (ld_dkv), each row written exactly once; deterministic, and
+ * bit-identical per sample to dllm_attn_bwd_gqa on that sample alone.  The workspace holds delta and lse * log2(e) as two [nh, T_pad]
+ * fp32 planes, T_pad = round_up(T, 64) + 64 (the backward reads whole 64-row tiles: the slack after row T is written as zeros). */
+size_t dllm_attn_bwd_varlen_workspace_bytes(int T, int nh, int d);
+int dllm_attn_bwd_varlen(const void* dout, const void* q, const void* k, const void* v, const void* out, const float* lse, void* dq,
+                         void* dk, void* dv, const int* cu_seqlens, void* workspace, size_t workspace_bytes, int B, int T, int max_seqlen,
+                         int nh, int nkv, int d, long ld_q, long ld_kv, long ld_o, long ld_dq, long ld_dkv, int causal, float scale,
+                         void* stream);
 /* ResnetBlock2D / Upsample2D conv: implicit-GEMM 3x3 stride-1 pad-1 on wgmma tensor cores (4-D TMA im2col, zero-fill padding).
  * y = conv(x, w) + bias[c] + rowbias[n, c] (+ residual);  w is [Cout, 3, 3, Cin]. */
 int dllm_conv3x3_nhwc(const void* x, const void* w, void* y, int N, int H, int W, int Cin, int Cout, const void* bias,
