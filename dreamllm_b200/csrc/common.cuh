@@ -105,6 +105,12 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
+// four 8 x 8 b16 blocks from the mma accumulator fragment layout (thread i: row i / 4, elements 2 (i % 4), + 1 of each block) to shared
+// memory; lanes 8 b .. 8 b + 7 give the addresses of the rows of block b (16 bytes each).  No "memory" clobber: volatile keeps it in
+// order with the fences and barriers around it, and global loads may move across it.  Nothing reads what it wrote through C++.
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3));
+}
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)

@@ -12,8 +12,10 @@
 // Structure (one CTA of 384 threads per SM, persistent over a static tile list: CTA c takes tiles c, c + grid, ...):
 //   warpgroup 0     TMA producer (one elected thread): global -> 128B-swizzled smem stages, mbarrier complete_tx
 //   warpgroups 1-2  consumers: each issues wgmma.mma_async (m64 x kBN x k16) for its 64 rows of the 128-row tile, keeps the fp32
-//                   accumulator in registers and runs the epilogue from registers straight to global memory.  The producer keeps
-//                   filling stages for the next tile meanwhile.
+//                   accumulator in registers and runs the epilogue.  bf16 outputs are staged in shared memory 64 columns at a time
+//                   and leave as TMA bulk tensor stores that drain while the warpgroup goes on (kStaged); fp32 outputs, and bf16
+//                   views no tensor map can describe, are stored from registers.  The producer keeps filling stages for the next
+//                   tile meanwhile.
 //   setmaxnreg moves registers from the producer warpgroup to the consumers (a 64 x 256 fp32 accumulator is 128 registers a thread).
 #include <stdlib.h>
 
@@ -28,17 +30,25 @@ constexpr int BN = 256;  // widest N tile (kBN 128 / 160 / 192 / 224 are instant
 constexpr int BK = 64;   // 64 bf16 = one 128-byte swizzle line
 constexpr int kGemmThreads = 384;
 
-template <int kBN = BN>
+template <int kBN = BN, bool kStaged = false>
 struct GemmCfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = kBN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kBarBytes = 256;
-  // operand stages + barriers <= 227 KB:  kBN 256: 4 stages, 224 / 192: 5, 160: 6, 128: 7 (every stage size is a multiple of the
-  // 1 KB the 128-byte swizzle needs as alignment)
-  static constexpr int kStagesFit = (227 * 1024 - kBarBytes - 1024) / kStageBytes;
+  // staged epilogue: two 8 KB buffers (64 rows x 64 bf16 columns) per consumer warpgroup, one being filled while the other drains
+  static constexpr int kOutBufBytes = 64 * 64 * 2;
+  static constexpr int kOutBytes = kStaged ? 2 * 2 * kOutBufBytes : 0;
+  // operand stages + staging + barriers <= 227 KB (every stage size is a multiple of the 1 KB the 128-byte swizzle needs as alignment):
+  //   kBN        256  224  192  160  128
+  //   direct       4    5    5    6    7
+  //   staged       4    4    4    5    6
+  static constexpr int kStagesFit = (227 * 1024 - kBarBytes - 1024 - kOutBytes) / kStageBytes;
   static constexpr int kStages = kStagesFit > 8 ? 8 : kStagesFit;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024 /*align slack*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + kBarBytes + 1024 /*align slack*/;
+  // a staging buffer leaves as one 64-column box (128-byte swizzle); widths that end in half a buffer (160, 224) use 32-column boxes
+  // (64-byte swizzle), two to a buffer, so that the last one stops at the tile's edge
+  static constexpr int kBoxCols = (kBN % 64) ? 32 : 64;
 };
 
 // Fused epilogue:  out = act( bf16(acc + bias[col]) ) (+ residual[row, col])   — rounding points as the reference's
@@ -88,22 +98,66 @@ __device__ __forceinline__ void store2(OutT* C, long ldc, int row, int col, int 
   }
 }
 
+__device__ __forceinline__ float2 bf16x2_f(uint32_t v) { return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v)); }
+__device__ __forceinline__ uint32_t ld_u32(const bf16* p) { return *reinterpret_cast<const uint32_t*>(p); }
+
+// The fused epilogue's arithmetic on two adjacent columns, shared by the direct and the staged store paths (kEpi 1 / 2).
+template <int kEpi>
+__device__ __forceinline__ void epi_apply(float& x0, float& x1, float2 bb, bool has_rb, float2 rb, int act, bool has_rs, float2 rs) {
+  x0 += bb.x;
+  x1 += bb.y;
+  if (has_rb) {
+    x0 += rb.x;
+    x1 += rb.y;
+  }
+  if constexpr (kEpi == 2) {
+    x0 = bf16_round(x0);
+    x1 = bf16_round(x1);
+    if (act == 1) {
+      x0 = x0 / (1.f + __expf(-1.702f * x0));
+      x1 = x1 / (1.f + __expf(-1.702f * x1));
+    } else if (act == 2) {
+      x0 = 0.5f * x0 * (1.f + erff(x0 * 0.70710678118654752f));
+      x1 = 0.5f * x1 * (1.f + erff(x1 * 0.70710678118654752f));
+    } else {
+      x0 = x0 / (1.f + __expf(-x0));
+      x1 = x1 / (1.f + __expf(-x1));
+    }
+  }
+  if (has_rs) {
+    x0 = bf16_round(x0) + rs.x;
+    x1 = bf16_round(x1) + rs.y;
+  }
+}
+// GEGLU on one element: value and gate pre-activations (accumulator + bias) -> h * gelu(gate), each factor rounded to bf16
+__device__ __forceinline__ float epi_geglu(float a, float g) {
+  a = bf16_round(a);
+  g = bf16_round(g);
+  return a * bf16_round(0.5f * g * (1.f + erff(g * 0.70710678118654752f)));
+}
+
 // kEpi: 0 = plain store, 1 = + bias / row-group bias / residual, 2 = 1 + activation, 3 = GEGLU.  Compile-time so that the plain and
 // the bias-only epilogues carry none of the (inlined expf / erff) activation code.
 //
 // ksplit > 1 (split-K, small-M shapes that would leave most SMs idle): a work unit is (output tile, K slice); unit u covers K blocks
 // [ks * kb_per, min(num_kb, (ks + 1) * kb_per)) of tile u / ksplit and stores its fp32 partial at rows ks * Mp + ... of C (the
 // workspace; Mp = M rounded up to whole tiles); splitk_reduce_kernel sums the slices and applies the epilogue.
-template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN>
+//
+// kStaged (bf16 outputs): the epilogue's results go to shared memory and leave through tma_c, the tensor map of the output view
+// ([M, N] at pitch ldc; [M, N / 2] for GEGLU), which clips at the view's extents: no row or column test guards a store.
+template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN, bool kStaged = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, OutT* __restrict__ C, long ldc,
-            int M, int N, int K, int group_m, GemmEpi epi, ConvGeom cg, int ksplit) {
-  using Cfg = GemmCfg<kBN>;
+gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+            const __grid_constant__ CUtensorMap tma_c, OutT* __restrict__ C, long ldc, int M, int N, int K, int group_m, GemmEpi epi,
+            ConvGeom cg, int ksplit) {
+  static_assert(!kStaged || sizeof(OutT) == 2, "staged epilogue: bf16 out");
+  using Cfg = GemmCfg<kBN, kStaged>;
   constexpr int kStages = Cfg::kStages;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+  uint8_t* out_s = smem + kStages * Cfg::kStageBytes;   // staging buffers [warpgroup][2] (kStaged)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(out_s + Cfg::kOutBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
 
@@ -112,6 +166,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
+    if constexpr (kStaged) tma_prefetch_desc(&tma_c);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
@@ -197,6 +252,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     const uint64_t adesc0 = kAMN ? make_smem_desc(a_s0, 8192, 1024) : make_smem_desc(a_s0, 16, 1024);
     const uint64_t bdesc0 = kBMN ? make_smem_desc(b_s0, 8192, 1024) : make_smem_desc(b_s0, 16, 1024);
     constexpr uint32_t a_step = kAMN ? 2048u : 32u, b_step = kBMN ? 2048u : 32u;   // bytes per K = 16 step
+    const uint32_t a_lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(adesc0), 0), a_hi = static_cast<uint32_t>(adesc0 >> 32);
+    const uint32_t b_lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(bdesc0), 0), b_hi = static_cast<uint32_t>(bdesc0 >> 32);
+    // staged epilogue: stmatrix.x4 writes four 8 x 8 blocks (two 8-column groups x two 8-row halves) of the warp's 16 rows; lane l
+    // supplies the address of row l % 8 of block l / 8.  A buffer row is 128 bytes (64 in the 32-column boxes) and its 16-byte chunks
+    // are XOR-swizzled by the row as the TMA box expects, which also spreads the 8 rows of a block over all 32 banks.
+    const int st_r = 16 * (t >> 5) + 8 * ((lane >> 3) & 1) + (lane & 7);
+    const uint32_t st_row = st_r * (Cfg::kBoxCols == 64 ? 128 : 64);
+    const uint32_t st_xor = ((lane >> 4) ^ (Cfg::kBoxCols == 64 ? (st_r & 7) : ((st_r >> 1) & 3))) << 4;
+    int sbuf = 0;   // staging buffer the next 64 columns go to
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -207,25 +271,139 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase, 3);
-        const uint64_t soff = static_cast<uint64_t>((stage * Cfg::kStageBytes) >> 4);
-        const uint64_t da = adesc0 + soff, db = bdesc0 + soff;
+        // only the low word of a descriptor (start address, leading offset) changes with the stage and the K step, and the sum never
+        // carries out of it.  The words are broadcast from lane 0, which tells the compiler they are the same across the warp: the
+        // adds run on the uniform datapath, where wgmma takes its descriptors from, and the group's MMAs issue back to back.
+        const uint32_t soff = __shfl_sync(0xffffffffu, static_cast<uint32_t>((stage * Cfg::kStageBytes) >> 4), 0);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          wgmma_ss<kBN, kAMN ? 1 : 0, kBMN ? 1 : 0>(acc, da + ((k * a_step) >> 4), db + ((k * b_step) >> 4), (kb != kb0 || k != 0) ? 1 : 0);
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t da = (static_cast<uint64_t>(a_hi) << 32) | (a_lo + soff + ((k * a_step) >> 4));
+          const uint64_t db = (static_cast<uint64_t>(b_hi) << 32) | (b_lo + soff + ((k * b_step) >> 4));
+          wgmma_ss<kBN, kAMN ? 1 : 0, kBMN ? 1 : 0>(acc, da, db, (kb != kb0 || k != 0) ? 1 : 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();   // the previous K block's MMAs have retired: its stage can be refilled
         if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         prev = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      const int row_t = m_blk * BM + wg * 64 + r_in;        // + 8h
+      const int col_t = n_blk * kBN + c_in;                 // + 8j
+      if constexpr (kStaged) {
+        // ---- epilogue: registers -> swizzled staging buffer -> TMA store, one buffer (64 output columns, 8 groups of 8) at a time ----
+        constexpr int kJ = (kEpi == 3) ? kBN / 16 : kBN / 8;        // 8-column groups of the output tile
+        constexpr int kBufs = (kJ + 7) / 8;
+        const int ncols = (kEpi == 3) ? (N >> 1) : N;
+        const int ocol0 = (kEpi == 3) ? n_blk * (kBN / 2) : n_blk * kBN;
+        const int orow0 = m_blk * BM + wg * 64;
+        const bool live = orow0 < M;                                 // the same for the whole warpgroup
+        const bool has_rb = kEpi > 0 && epi.rowbias != nullptr, has_rs = kEpi > 0 && epi.residual != nullptr;
+        const bf16* rbp[2] = {nullptr, nullptr};
+        const bf16* rsp[2] = {nullptr, nullptr};
+        if constexpr (kEpi == 1 || kEpi == 2) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row_t + 8 * h;
+            if (has_rb && row < M) rbp[h] = epi.rowbias + static_cast<size_t>(row / epi.rows_per_group) * N;
+            if (has_rs && row < M) rsp[h] = epi.residual + static_cast<size_t>(row) * epi.ldr;
+          }
+        }
+        // the epilogue's operands of the two 8-column groups jj, jj + 1 of buffer u, as raw bf16 pairs: bias (GEGLU: value bias),
+        // row-group bias (GEGLU: gate bias in rb[0]), residual.  The first two groups' are fetched while the last K blocks retire (kEarly);
+        // the rest are independent loads the compiler is free to issue ahead of the arithmetic (stmatrix does not order them).
+        struct EpiIn { uint32_t b[2], rb[2][2], rs[2][2]; };
+        auto epi_load = [&](int u, int jj0, EpiIn& in) {
+          if constexpr (kEpi != 0) {
+#pragma unroll
+            for (int dj = 0; dj < 2; ++dj) {
+              if constexpr (kEpi == 3) {
+                const int col = col_t + 128 * u + 8 * (jj0 + dj);  // value column in the permuted N space (gate at + 64)
+                const bool ok = epi.bias != nullptr && col < N;
+                in.b[dj] = ok ? ld_u32(epi.bias + col) : 0u;
+                in.rb[0][dj] = ok ? ld_u32(epi.bias + col + 64) : 0u;
+              } else {
+                const int col = col_t + 64 * u + 8 * (jj0 + dj);
+                const bool ok = col < N;                             // fused epilogues require N % 8 == 0
+                in.b[dj] = (ok && epi.bias != nullptr) ? ld_u32(epi.bias + col) : 0u;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  in.rb[h][dj] = (ok && rbp[h] != nullptr) ? ld_u32(rbp[h] + col) : 0u;
+                  in.rs[h][dj] = (ok && rsp[h] != nullptr) ? ld_u32(rsp[h] + col) : 0u;
+                }
+              }
+            }
+          }
+        };
+        constexpr bool kEarly = kBN <= 192;   // the 224 / 256-wide accumulators leave no registers to hold operands across the wait
+        EpiIn first;
+        if (kEarly && live) epi_load(0, 0, first);
+        wgmma_wait<0>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (live) {
+#pragma unroll
+          for (int u = 0; u < kBufs; ++u) {
+            const int c0 = ocol0 + 64 * u;
+            if (c0 >= ncols) break;
+            uint8_t* buf = out_s + (wg * 2 + sbuf) * Cfg::kOutBufBytes;
+            const uint32_t buf_u32 = smem_u32(buf);
+#pragma unroll
+            for (int jj = 0; jj < 8; jj += 2) {
+              if (8 * u + jj >= kJ) continue;
+              EpiIn cur;
+              if (kEarly && u == 0 && jj == 0) cur = first;
+              else epi_load(u, jj, cur);
+              uint32_t r[4];                                         // matrices (jj, h 0), (jj, h 1), (jj + 1, h 0), (jj + 1, h 1)
+#pragma unroll
+              for (int dj = 0; dj < 2; ++dj) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  float x0, x1;
+                  if constexpr (kEpi == 3) {
+                    const int j = 16 * u + jj + dj;
+                    const float2 bv = bf16x2_f(cur.b[dj]), bg = bf16x2_f(cur.rb[0][dj]);
+                    x0 = epi_geglu(acc[4 * j + 2 * h] + bv.x, acc[4 * (j + 8) + 2 * h] + bg.x);
+                    x1 = epi_geglu(acc[4 * j + 2 * h + 1] + bv.y, acc[4 * (j + 8) + 2 * h + 1] + bg.y);
+                  } else {
+                    const int j = 8 * u + jj + dj;
+                    x0 = acc[4 * j + 2 * h];
+                    x1 = acc[4 * j + 2 * h + 1];
+                    if constexpr (kEpi > 0)
+                      epi_apply<kEpi>(x0, x1, bf16x2_f(cur.b[dj]), has_rb, bf16x2_f(cur.rb[h][dj]), epi.act, has_rs,
+                                      bf16x2_f(cur.rs[h][dj]));
+                  }
+                  r[2 * dj + h] = pack_bf16(x0, x1);
+                }
+              }
+              const uint32_t off = Cfg::kBoxCols == 64 ? st_row + ((jj << 4) ^ st_xor)
+                                                       : (jj >> 2) * 4096 + st_row + (((jj & 3) << 4) ^ st_xor);
+              stmatrix_x4(buf_u32 + off, r[0], r[1], r[2], r[3]);
+            }
+            // every thread's writes become visible to the TMA engine; thread 0 has seen the previous store (the other buffer) read
+            // its source, so past the barrier that buffer is free for u + 1
+            fence_proxy_async_smem();
+            if (t == 0) tma_store_wait_read<0>();
+            named_bar_sync(1 + wg, 128);
+            if (t == 0) {
+              if constexpr (Cfg::kBoxCols == 64) {
+                tma_store_2d(&tma_c, buf, c0, orow0);
+              } else {
+#pragma unroll
+                for (int k = 0; k < 2; ++k)
+                  if (8 * u + 4 * k < kJ && c0 + 32 * k < ncols) tma_store_2d(&tma_c, buf + 4096 * k, c0 + 32 * k, orow0);
+              }
+              tma_store_commit();
+            }
+            sbuf ^= 1;
+          }
+        }
+      } else {
       wgmma_wait<0>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      // ---- epilogue: registers -> global ----
-      const int row_t = m_blk * BM + wg * 64 + r_in;        // + 8h
-      const int col_t = n_blk * kBN + c_in;                 // + 8j
+      // ---- epilogue: registers -> global (fp32 outputs; bf16 views whose base or pitch a tensor map cannot take) ----
       const long row_off = (ksplit > 1) ? static_cast<long>(ks) * split_rows : 0;
+      const bool pair_ok = (ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(C) & (2 * sizeof(OutT) - 1)) == 0;
       if constexpr (kEpi == 3) {
         // GEGLU epilogue (diffusers FeedForward: h, gate = proj(x).chunk(2); out = h * gelu(gate)).  The weight rows were permuted at
         // load time so that every 128-column group of this GEMM's N space is [64 value columns | their 64 gate columns]; a thread
@@ -247,25 +425,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             for (int h = 0; h < 2; ++h) {
               const int row = row_t + 8 * h;
               if (row >= M) continue;
-              float o[2];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float a = bf16_round(acc[4 * j + 2 * h + e] + (e ? bv.y : bv.x));
-                const float gte = bf16_round(acc[4 * (j + 8) + 2 * h + e] + (e ? bg.y : bg.x));
-                const float gel = bf16_round(0.5f * gte * (1.f + erff(gte * 0.70710678118654752f)));
-                o[e] = a * gel;
-              }
-              store2<OutT>(C, ldc, row, ocol, N >> 1, !(ldc & 1), o[0], o[1]);
+              const float o0 = epi_geglu(acc[4 * j + 2 * h] + bv.x, acc[4 * (j + 8) + 2 * h] + bg.x);
+              const float o1 = epi_geglu(acc[4 * j + 2 * h + 1] + bv.y, acc[4 * (j + 8) + 2 * h + 1] + bg.y);
+              store2<OutT>(C, ldc, row, ocol, N >> 1, pair_ok, o0, o1);
             }
           }
         }
       } else {
-        const bool even_ld = (ldc & 1) == 0;
 #pragma unroll
         for (int j = 0; j < kBN / 8; ++j) {
           const int col = col_t + 8 * j;
           if (col >= N) continue;
-          const bool pair = even_ld && col + 1 < N;
+          const bool pair = pair_ok && col + 1 < N;
           float2 bb = make_float2(0.f, 0.f);
           if (kEpi > 0 && epi.bias != nullptr) bb = ld_bf16x2(epi.bias + col);   // fused epilogues require N % 8 == 0
 #pragma unroll
@@ -274,37 +445,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             if (row >= M) continue;
             float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
             if constexpr (kEpi > 0) {
-              x0 += bb.x;
-              x1 += bb.y;
-              if (epi.rowbias != nullptr) {
-                const float2 rb = ld_bf16x2(epi.rowbias + static_cast<size_t>(row / epi.rows_per_group) * N + col);
-                x0 += rb.x;
-                x1 += rb.y;
-              }
-              if constexpr (kEpi == 2) {
-                x0 = bf16_round(x0);
-                x1 = bf16_round(x1);
-                if (epi.act == 1) {
-                  x0 = x0 / (1.f + __expf(-1.702f * x0));
-                  x1 = x1 / (1.f + __expf(-1.702f * x1));
-                } else if (epi.act == 2) {
-                  x0 = 0.5f * x0 * (1.f + erff(x0 * 0.70710678118654752f));
-                  x1 = 0.5f * x1 * (1.f + erff(x1 * 0.70710678118654752f));
-                } else {
-                  x0 = x0 / (1.f + __expf(-x0));
-                  x1 = x1 / (1.f + __expf(-x1));
-                }
-              }
-              if (epi.residual != nullptr) {
-                const float2 rs = ld_bf16x2(epi.residual + static_cast<size_t>(row) * epi.ldr + col);
-                x0 = bf16_round(x0) + rs.x;
-                x1 = bf16_round(x1) + rs.y;
-              }
+              float2 rb = make_float2(0.f, 0.f), rs = make_float2(0.f, 0.f);
+              if (epi.rowbias != nullptr) rb = ld_bf16x2(epi.rowbias + static_cast<size_t>(row / epi.rows_per_group) * N + col);
+              if (epi.residual != nullptr) rs = ld_bf16x2(epi.residual + static_cast<size_t>(row) * epi.ldr + col);
+              epi_apply<kEpi>(x0, x1, bb, epi.rowbias != nullptr, rb, epi.act, epi.residual != nullptr, rs);
             }
             store2<OutT>(C, ldc, static_cast<int>(row + row_off), col, N, pair, x0, x1);
           }
         }
       }
+      }
+    }
+    if constexpr (kStaged) {
+      if (t == 0) tma_store_wait_all<0>();   // the last stores have left shared memory and reached global memory before the CTA exits
     }
   }
 }
@@ -341,6 +494,25 @@ int make_tmap_2d(CUtensorMap* map, const void* ptr, int elem_bytes, uint64_t row
   if (r != CUDA_SUCCESS)
     fprintf(stderr, "dllm: cuTensorMapEncodeTiled failed (CUresult %d): ptr=%p elem=%d rows=%llu cols=%llu ld=%llu box=[%u x %u]\n",
             (int)r, ptr, elem_bytes, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, box_cols);
+  return r == CUDA_SUCCESS ? 0 : DLLM_ERR_TMAP;
+}
+
+// Output view [rows, cols] of bf16 at pitch `ld`, written in boxes of 64 rows x 32 | 64 columns (64- | 128-byte swizzle).  The extents
+// are the view's, not the allocation's: the TMA store clips at them, and that is all that keeps a tile's tail rows and columns from
+// being written.
+static int make_tmap_out(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_cols) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return DLLM_ERR_DRIVER;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstr[1] = {ld * 2};
+  cuuint32_t box[2] = {box_cols, 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    fprintf(stderr, "dllm: cuTensorMapEncodeTiled(out) failed (CUresult %d): ptr=%p rows=%llu cols=%llu ld=%llu box=[64 x %u]\n", (int)r,
+            ptr, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_cols);
   return r == CUDA_SUCCESS ? 0 : DLLM_ERR_TMAP;
 }
 
@@ -412,11 +584,15 @@ static int plan_bn(int M, int N, int a_mn, int b_mn, bool bf16_out) {
   return w[0].bn;
 }
 
-template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN>
+template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0, int kBN = BN, bool kStaged = false>
 static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
                           cudaStream_t stream, ConvGeom cg = ConvGeom{1, 1, 1, 1}, int ksplit = 1) {
-  using Cfg = GemmCfg<kBN>;
-  auto kern = gemm_kernel<kAMN, kBMN, OutT, kConv, kEpi, kBN>;
+  using Cfg = GemmCfg<kBN, kStaged>;
+  auto kern = gemm_kernel<kAMN, kBMN, OutT, kConv, kEpi, kBN, kStaged>;
+  CUtensorMap tc{};
+  if constexpr (kStaged) {
+    if (int rc = make_tmap_out(&tc, C, M, kEpi == 3 ? N / 2 : N, ldc, Cfg::kBoxCols)) return rc;
+  }
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess)
@@ -427,22 +603,33 @@ static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, void* C,
   int avail = num_sms() - g_reserved_sms;
   if (avail < 1) avail = 1;
   const int grid = num_tiles < avail ? num_tiles : avail;
-  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, static_cast<OutT*>(C), ldc, M, N, K, 16, epi, cg, ksplit);
+  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, tc, static_cast<OutT*>(C), ldc, M, N, K, 16, epi, cg, ksplit);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+// bf16 outputs take the staged (TMA store) epilogue whenever a tensor map can describe the view: base 16-byte aligned, row pitch a
+// multiple of 16 bytes.  Any other bf16 view, and every fp32 output, is stored from registers.
+template <bool kAMN, bool kBMN, typename OutT, bool kConv, int kEpi, int kBN>
+static int launch_gemm_out(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
+                           cudaStream_t stream, ConvGeom cg) {
+  if constexpr (sizeof(OutT) == 2) {
+    if (!(reinterpret_cast<uintptr_t>(C) & 15) && !(ldc & 7))
+      return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, kBN, true>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  }
+  return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, kBN, false>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
 }
 // `bn` must be the value the B tensor map's box was built for (plan_bn); only the widths plan_bn can return are instantiated
 template <bool kAMN, bool kBMN, typename OutT, bool kConv = false, int kEpi = 0>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, long ldc, int M, int N, int K, const GemmEpi& epi,
                        cudaStream_t stream, ConvGeom cg, int bn) {
   if constexpr (!kAMN && sizeof(OutT) == 2) {
-    if (bn == 192) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 192>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+    if (bn == 192) return launch_gemm_out<kAMN, kBMN, OutT, kConv, kEpi, 192>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
     if constexpr (!kBMN) {
-      if (bn == 160) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 160>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
-      if (bn == 224) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 224>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+      if (bn == 160) return launch_gemm_out<kAMN, kBMN, OutT, kConv, kEpi, 160>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+      if (bn == 224) return launch_gemm_out<kAMN, kBMN, OutT, kConv, kEpi, 224>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
     }
   }
-  if (bn == 128) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 128>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
-  if (bn == 256) return launch_gemm_bn<kAMN, kBMN, OutT, kConv, kEpi, 256>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  if (bn == 128) return launch_gemm_out<kAMN, kBMN, OutT, kConv, kEpi, 128>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
+  if (bn == 256) return launch_gemm_out<kAMN, kBMN, OutT, kConv, kEpi, 256>(ta, tb, C, ldc, M, N, K, epi, stream, cg);
   return DLLM_ERR_UNSUPPORTED;
 }
 
@@ -536,7 +723,9 @@ static int launch_splitk_reduce(const void* ws, void* out, long ldc, int M, int 
 int gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, long lda, long ldb, long ldc, int b_mn, const void* bias,
                  const void* residual, long ldr, int act, void* ws, size_t ws_bytes, cudaStream_t stream) {
   const SplitPlan p = plan_split(M, N, K);
-  if (p.ksplit <= 1 || !ws || ws_bytes < p.ws_bytes || (N % 8) || (reinterpret_cast<uintptr_t>(ws) & 15) || (ldc % 8))
+  // (the reduce kernel writes 16 bytes at a time: an output view it cannot write that way runs unsplit)
+  if (p.ksplit <= 1 || !ws || ws_bytes < p.ws_bytes || (N % 8) || (reinterpret_cast<uintptr_t>(ws) & 15) || (ldc % 8) ||
+      (reinterpret_cast<uintptr_t>(C) & 15))
     return gemm_bf16_ex(A, B, C, M, N, K, lda, ldb, ldc, 0, b_mn, 0, -1, bias, residual, ldr, act, stream);
   if (residual && ((reinterpret_cast<uintptr_t>(residual) & 15) || ((ldr * 2) & 15))) return DLLM_ERR_ALIGN;
   if (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) return DLLM_ERR_ALIGN;
@@ -571,7 +760,7 @@ int gemm_bf16_ex(const void* A, const void* B, void* C, int M, int N, int K, lon
   if ((bias || residual) && (N % 8)) return DLLM_ERR_SHAPE;
   if (residual && ((reinterpret_cast<uintptr_t>(residual) & 15) || ((ldr * 2) & 15))) return DLLM_ERR_ALIGN;
   if (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) return DLLM_ERR_ALIGN;
-  if (reinterpret_cast<uintptr_t>(C) & 15) return DLLM_ERR_ALIGN;
+  if (reinterpret_cast<uintptr_t>(C) & (out_fp32 ? 15 : 1)) return DLLM_ERR_ALIGN;   // bf16: see launch_gemm_out
   GemmEpi epi{static_cast<const bf16*>(bias), static_cast<const bf16*>(residual), ldr, act, nullptr, 1};
   const int bn = plan_bn(M, N, a_mn, b_mn, !out_fp32);
   const ConvGeom nocg{1, 1, 1, 1};
@@ -612,13 +801,13 @@ int gemm_bf16_geglu(const void* A, const void* Wp, const void* bias_p, void* out
                     cudaStream_t stream) {
   if (M <= 0 || N <= 0 || K <= 0 || (N % 128)) return DLLM_ERR_SHAPE;
   if (bias_p && (reinterpret_cast<uintptr_t>(bias_p) & 15)) return DLLM_ERR_ALIGN;
-  if (reinterpret_cast<uintptr_t>(out) & 15) return DLLM_ERR_ALIGN;
+  if (reinterpret_cast<uintptr_t>(out) & 1) return DLLM_ERR_ALIGN;
   GemmEpi epi{static_cast<const bf16*>(bias_p), nullptr, 0, 2, nullptr, 1};
   CUtensorMap ta, tb;
   int rc;
   if ((rc = make_tmap_2d(&ta, A, 2, M, K, lda, BM, BK))) return rc;
   if ((rc = make_tmap_2d(&tb, Wp, 2, N, K, ldb, BN, BK))) return rc;
-  return launch_gemm_bn<false, false, bf16, false, 3, 256>(ta, tb, out, ldc, M, N, K, epi, stream);
+  return launch_gemm_out<false, false, bf16, false, 3, 256>(ta, tb, out, ldc, M, N, K, epi, stream, ConvGeom{1, 1, 1, 1});
 }
 
 // 4-D NHWC activation map: dims {C, W, H, N}, box {64, Wb, Hb, Nb}, 128B swizzle.
@@ -651,7 +840,7 @@ int conv3x3_nhwc_ws(const void* x, const void* w, void* y, int Nimg, int H, int 
                     const void* rowbias, const void* residual, void* ws, size_t ws_bytes, cudaStream_t stream) {
   if (Nimg <= 0 || Cin % 64 || Cout % 8) return DLLM_ERR_SHAPE;
   if (W > 128 ? (W % 128) : (128 % W)) return DLLM_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(y) & 15) return DLLM_ERR_ALIGN;
+  if (reinterpret_cast<uintptr_t>(y) & 1) return DLLM_ERR_ALIGN;
   const int HW = H * W;
   int Wb = W > 128 ? 128 : W, Hb = W > 128 ? 1 : 128 / W, Nb = 1;
   if (Hb > H) {  // small planes: the 128-pixel tile spans several whole images
@@ -663,7 +852,8 @@ int conv3x3_nhwc_ws(const void* x, const void* w, void* y, int Nimg, int H, int 
   }
   const int M = Nimg * HW, K = 9 * Cin;
   const SplitPlan sp = plan_split(M, Cout, K);
-  const bool split = sp.ksplit > 1 && ws && ws_bytes >= sp.ws_bytes && !(reinterpret_cast<uintptr_t>(ws) & 15);
+  const bool split = sp.ksplit > 1 && ws && ws_bytes >= sp.ws_bytes && !(reinterpret_cast<uintptr_t>(ws) & 15) &&
+                     !(reinterpret_cast<uintptr_t>(y) & 15);
   const int bn = split ? sp.bn : plan_bn(M, Cout, 0, 0, true);
   CUtensorMap ta, tb;
   int rc;

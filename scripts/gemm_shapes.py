@@ -4,7 +4,10 @@
                                             per (M, N, K, mode) group, largest time first
   python scripts/gemm_shapes.py widths      the fixed c5 shape table below, timed with CUDA events over many launches, once per N-tile
                                             width (DLLM_GEMM_BN pins the width; one child process per width) and once as planned
-  python scripts/gemm_shapes.py all         both
+  python scripts/gemm_shapes.py tilecost    the same table plus two VAE-encoder convolutions and one split-K linear, each timed at K and at
+                                            2K (same M, N and width): fixed = 2 t(K) - t(2K) is the part of the launch that does not scale
+                                            with K (tile prologue + epilogue), printed per wave of tiles next to t(K)
+  python scripts/gemm_shapes.py all         profile and widths
 
 Runs on whichever library DLLM_LIB_PATH names (default: the in-tree build), so two builds can be compared side by side.  A build older
 than the tile planner ignores DLLM_GEMM_BN and has no dllm_gemm_tile_n; its rows then all show its own fixed widths.
@@ -46,6 +49,9 @@ SHAPES = [
     ("conv", 16384, 320, 9 * 320), ("conv", 16384, 320, 9 * 640), ("conv", 4096, 640, 9 * 640), ("conv", 4096, 640, 9 * 1280),
 ]
 WIDTHS = (256, 224, 192, 160, 128)
+# tilecost only: VAE encoder 3x3 convolutions at the full- and half-resolution levels of 4 images of 512x512, and the UNet's 16x16-level
+# linear (a split-K launch: its fixed part includes the fp32 partial store and the reduce kernel)
+TILECOST_EXTRA = [("conv", 4 * 512 * 512, 128, 9 * 128), ("conv", 4 * 256 * 256, 256, 9 * 256), ("fwd", 1024, 1280, 1280)]
 
 
 def _time(fn, iters):
@@ -79,6 +85,34 @@ def _bench_one(kind, M, N, K):
     flop = 2.0 * M * N * K
     iters = max(20, min(2000, int(2e13 / flop)))     # ~ 20 ms of work per timing
     return min(_time(fn, iters) for _ in range(3))
+
+
+def _card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(0)
+
+
+def tilecost():
+    L = _load()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    print(f"\ncard: {_card()}; {sms} SMs")
+    print("fixed = 2 t(K) - t(2K): the time of a launch that does not scale with K; per wave = fixed / ceil(tiles / SMs)")
+    print(f"{'kind':6s} {'M':>8s} {'N':>6s} {'K':>6s} {'bn':>4s} {'waves':>5s} | {'t(K) us':>9s} {'t(2K) us':>9s} | {'fixed us':>9s} "
+          f"{'per wave':>9s} {'of t(K)':>8s}")
+    for kind, M, N, K in SHAPES + TILECOST_EXTRA:
+        b_mn = int(kind == "dgrad")
+        bn = L.dllm_gemm_tile_n(M, N, K, b_mn)
+        if L.dllm_gemm_tile_n(M, N, 2 * K, b_mn) != bn:
+            raise RuntimeError(f"{(kind, M, N, K)}: K and 2K plan different widths")
+        split = "*" if M <= 4096 and L.dllm_gemm_splitk_workspace_bytes(M, N, K) else " "
+        t1 = _bench_one(kind, M, N, K) * 1e3
+        t2 = _bench_one(kind, M, N, 2 * K) * 1e3
+        waves = -(-((M + 127) // 128 * -(-N // bn)) // sms)
+        fixed = 2 * t1 - t2
+        print(f"{kind:6s} {M:8d} {N:6d} {K:6d} {bn:4d} {waves:5d} | {t1:9.1f} {t2:9.1f} | {fixed:9.1f} {fixed / waves:9.2f} "
+              f"{100 * fixed / t1:7.1f}%{split}")
+    print("* split-K launch (fp32 partials + reduce kernel)")
 
 
 def widths_child():
@@ -171,3 +205,5 @@ if __name__ == "__main__":
         profile()
     if what in ("widths", "all"):
         widths()
+    if what == "tilecost":
+        tilecost()
