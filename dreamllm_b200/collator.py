@@ -80,6 +80,11 @@ class DataCollatorForDreamLLMDataset:
         images_dm = torch.cat(images_dm, 0) if len(images_dm) > 0 else None
         out = dict(batch)
         out.update(input_ids=ids, attention_mask=mask, labels=labels, images=images, images_dm=images_dm)
+        if "add_time_ids" in batch:
+            # SDXL micro-conditioning: [n, 6] per example, concatenated in batch order, None if no example has any
+            # (reference builder_dreamllm.py:452-453, :501-502)
+            add_time_ids = [torch.as_tensor(x).reshape(-1, 6) for x in batch["add_time_ids"] if x is not None]
+            out["add_time_ids"] = torch.cat(add_time_ids, 0) if len(add_time_ids) > 0 else None
 
         # ---- device index maps (the part the reference recomputes on the GPU with host syncs every step)
         seqlens = mask.sum(-1).to(torch.int32)

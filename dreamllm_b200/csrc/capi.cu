@@ -354,4 +354,27 @@ int dllm_sumsq_bf16(const void* x, long n, float* out, int accumulate, void* wor
   return sumsq_bf16(x, n, out, accumulate, workspace, workspace_bytes, S(stream));
 }
 
+size_t dllm_channel_sum_workspace_bytes(int N, int HW, int C) { return channel_sum_workspace(N, HW, C); }
+int dllm_channel_sum_nhwc(const void* x, void* out, long ldo, int out_bf16, float scale, int N, int HW, int C, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  ensure_context(x);
+  return channel_sum_nhwc(x, out, ldo, out_bf16, scale, N, HW, C, workspace, workspace_bytes, S(stream));
+}
+int dllm_time_ids_embedding(const float* ids, void* out, long ldo, int B, int n_ids, int dim, void* stream) {
+  ensure_context(out);
+  return time_ids_embedding(ids, out, ldo, B, n_ids, dim, S(stream));
+}
+int dllm_silu_bf16(const void* x, void* y, long n, void* stream) {
+  ensure_context(x);
+  return silu_bf16(x, y, n, S(stream));
+}
+int dllm_silu_bwd_bf16(const void* dy, const void* x, void* dx, long n, void* stream) {
+  ensure_context(dy);
+  return silu_bwd_bf16(dy, x, dx, n, S(stream));
+}
+int dllm_broadcast_rows(const void* src, void* dst, int B, int R, int H, float scale, void* stream) {
+  ensure_context(src);
+  return broadcast_rows(src, dst, B, R, H, scale, S(stream));
+}
+
 }  // extern "C"

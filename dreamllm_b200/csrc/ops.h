@@ -97,4 +97,12 @@ int adamw_step(const void* grad, void* master, void* mom, void* var, void* param
                double beta2, double eps, double weight_decay, int step, const float* sumsq, double max_norm, cudaStream_t s);
 size_t sumsq_workspace();
 int sumsq_bf16(const void* x, long n, float* out, int accumulate, void* workspace, size_t ws_bytes, cudaStream_t s);
+// sdxl_ops.cu: addition embedding of the SDXL UNet and its gradient path
+size_t channel_sum_workspace(int N, int HW, int C);
+int channel_sum_nhwc(const void* x, void* out, long ldo, int out_bf16, float scale, int N, int HW, int C, void* workspace,
+                     size_t ws_bytes, cudaStream_t s);
+int time_ids_embedding(const float* ids, void* out, long ldo, int B, int n_ids, int dim, cudaStream_t s);
+int silu_bf16(const void* x, void* y, long n, cudaStream_t s);
+int silu_bwd_bf16(const void* dy, const void* x, void* dx, long n, cudaStream_t s);
+int broadcast_rows(const void* src, void* dst, int B, int R, int H, float scale, cudaStream_t s);
 }  // namespace dllm

@@ -1135,13 +1135,24 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
     def forward(self, input_ids=None, images=None, images_dm=None, attention_mask=None, position_ids=None,
                 past_key_values=None, inputs_embeds=None, labels=None, use_cache=None, output_attentions=None,
                 output_hidden_states=None, return_dict=None, attention_mask_has_padding=None, input_ids_cpu=None,
-                splice_plan=None, sd_kwargs=None, seqlens=None, shifted_labels=None, cu_seqlens=None, max_seqlen=None, **kwargs):
+                splice_plan=None, sd_kwargs=None, seqlens=None, shifted_labels=None, cu_seqlens=None, max_seqlen=None, add_time_ids=None,
+                **kwargs):
         """reference :1353-1509.  `seqlens` / `shifted_labels` / `splice_plan` / `input_ids_cpu` are the collator's precomputed maps
         (dreamllm_b200/collator.py, SURVEY §8f row 3); without them they are derived here as the reference does.  Comprehension path: images -> CLIP -> splice -> LM loss.  Creation path: dream-query conditioning
         gather (:1401-1418, also returned in `additional_log_info["dream_conditioning"]`) -> optional null-prompt pass (:1420-1439) ->
         `stable_diffusion_head` loss (:1441); `sd_kwargs` forwards injected random draws to the head (tests).
         `cu_seqlens` / `max_seqlen`: a packed batch (`input_ids` / `labels` [1, T], DreamLLMModel._forward); labels derived here get -100
-        at the last token of every sample, so that no sample is asked to predict the next one's first token."""
+        at the last token of every sample, so that no sample is asked to predict the next one's first token.
+        `add_time_ids` [Nd, 6]: the SDXL head's micro-conditioning, one row per dream image (reference modeling_dreamllm_sdxl.py:1357,
+        :1440); required when an `StableDiffusionXLHead` is trained, refused for any other head."""
+        xl_head = False
+        if add_time_ids is not None or images_dm is not None:
+            from .modeling_plugins import StableDiffusionXLHead
+            xl_head = isinstance(getattr(self, "stable_diffusion_head", None), StableDiffusionXLHead)
+        if add_time_ids is not None and not xl_head:
+            raise ValueError("add_time_ids is the SDXL head's conditioning; this model's stable_diffusion_head is not a StableDiffusionXLHead")
+        if xl_head and self.training and images_dm is not None and add_time_ids is None:
+            raise ValueError("training the StableDiffusionXLHead needs add_time_ids [Nd, 6] (the collator emits them from the examples)")
         out = self.model(input_ids=input_ids, images=images, images_dm=images_dm, attention_mask=attention_mask,
                          position_ids=position_ids, past_key_values=past_key_values, inputs_embeds=inputs_embeds,
                          use_cache=use_cache, output_attentions=output_attentions, output_hidden_states=output_hidden_states,
@@ -1182,7 +1193,8 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
                 u_enc = None
                 if getattr(head, "drop_prob", None) is not None:                                         # (:1420-1439)
                     u_enc = self._null_prompt_states(Q)
-                vm_loss = head(images_dm, enc_h, u_enc, **(sd_kwargs or {}))   # (:1441) fewer <dream_start> than images_dm -> the head's assert, as the reference
+                xl = (add_time_ids,) if xl_head else ()
+                vm_loss = head(images_dm, enc_h, u_enc, *xl, **(sd_kwargs or {}))   # (:1441) fewer <dream_start> than images_dm -> the head's assert, as the reference
                 loss = vm_loss * self.loss_weight_vm + (loss if loss is not None else 0.0)               # (:1486-1488)
         info["vm_loss"] = vm_loss
         sched = getattr(self.config, "loss_scale_schedule", "none")                                   # (:1472-1477, :1489)

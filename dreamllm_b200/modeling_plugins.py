@@ -18,6 +18,7 @@ import torch.nn as nn
 from . import ops
 from .clip_vision import CLIPVisionConfigLite, CLIPVisionModel
 from .projector import build_projector
+from .unet import SDXL
 
 BF16 = torch.bfloat16
 
@@ -489,6 +490,8 @@ class StableDiffusionHead(MultimodalHead):
     `diffusion_name_or_path` may be a dict of UNet config overrides for random init (no checkpoints exist in the sandbox);
     a checkpoint directory is loaded through safetensors into the native module (identical key names).
     """
+    _unet_config = None         # UNet architecture of a checkpoint directory / base of a dict of overrides (None: SD-2.1)
+    _vae_config = None          # AutoencoderKL overrides (None: SD-2.1's)
 
     def __init__(self, diffusion_name_or_path=None, projector_type="linear", projector_depth: int = 1,
                  projector_name_or_path: str = None, pretrained_model_name_or_path: str = None, embed_hidden_size: int = 4096,
@@ -511,7 +514,7 @@ class StableDiffusionHead(MultimodalHead):
             raise ValueError("the native UNet is a frozen tower (freeze_unet=True in every shipped config)")
         if isinstance(diffusion_name_or_path, str):
             import glob
-            self.unet = UNet2DConditionModel()
+            self.unet = UNet2DConditionModel(self._unet_config)
             files = glob.glob(os.path.join(diffusion_name_or_path, "unet", "*.safetensors"))
             if not files:
                 raise FileNotFoundError(f"no unet/*.safetensors under {diffusion_name_or_path}")
@@ -520,8 +523,12 @@ class StableDiffusionHead(MultimodalHead):
         else:
             cfgd = dict(diffusion_name_or_path or {})
             vae_cfg = cfgd.pop("vae", None)
-            self.unet = UNet2DConditionModel(cfgd)
-        self.vae = AutoencoderKLEncoder(vae_cfg if not isinstance(diffusion_name_or_path, str) else None)
+            self.unet = UNet2DConditionModel(cfgd if self._unet_config is None else {**self._unet_config, **cfgd})
+        if isinstance(diffusion_name_or_path, str):
+            vae_cfg = None
+        if self._vae_config is not None:
+            vae_cfg = {**self._vae_config, **(vae_cfg or {})}
+        self.vae = AutoencoderKLEncoder(vae_cfg)
         if isinstance(diffusion_name_or_path, str):
             import glob
             from safetensors.torch import load_file
@@ -529,7 +536,7 @@ class StableDiffusionHead(MultimodalHead):
             if vf:
                 self.vae.load_state_dict(load_file(vf[0]), strict=False)      # decoder.* / post_quant_conv.* are not part of this path
         # decode half of the same AutoencoderKL (separate module so its keys stay `decoder.*` / `post_quant_conv.*`)
-        self.vae_decoder = AutoencoderKLDecoder(vae_cfg if not isinstance(diffusion_name_or_path, str) else None)
+        self.vae_decoder = AutoencoderKLDecoder(vae_cfg)
         if isinstance(diffusion_name_or_path, str) and vf:
             self.vae_decoder.load_state_dict(load_file(vf[0]), strict=False)
         self.vae_decoder.requires_grad_(False)
@@ -585,6 +592,20 @@ class StableDiffusionHead(MultimodalHead):
         not needed by our reducer and returns None."""
         if images is None and latents is None:
             return None
+        noisy, noise, t32, ac = self._noisy_latents(images, encoder_hidden_states, latents, noise, timesteps, vae_noise, offset_noise,
+                                                    perturbation_noise)
+        bsz = noisy.shape[0]
+        if u_encoder_hidden_states is not None and self.drop_prob is not None:      # train with classifier-free guidance (:539-543)
+            if drop_mask is None:
+                drop_mask = torch.bernoulli(torch.zeros(bsz) + self.drop_prob)       # drawn on the host, as the reference does (:541)
+            encoder_hidden_states = _CfgDropFn.apply(encoder_hidden_states, u_encoder_hidden_states.to(encoder_hidden_states.dtype),
+                                                     drop_mask.detach().to("cpu"))
+        cond = self.projector(encoder_hidden_states)[-1]
+        snr = None if self.snr_gamma is None else (ac, float(self.snr_gamma))
+        return _DiffusionLossFn.apply(cond, self.unet, noisy, t32, noise, snr)      # epsilon prediction (:548-549)
+
+    def _noisy_latents(self, images, encoder_hidden_states, latents, noise, timesteps, vae_noise, offset_noise, perturbation_noise):
+        """VAE encode -> noise (+ offset, perturbation) -> timesteps -> add_noise.  Returns (noisy, target noise, t int32, alphas_cumprod)."""
         dev = encoder_hidden_states.device
         if latents is None:
             latents = self.vae.encode_sample(images, z=vae_noise)
@@ -610,14 +631,7 @@ class StableDiffusionHead(MultimodalHead):
         t32 = timesteps.to(torch.int32).contiguous()
         ac = self._alphas_cumprod(dev)
         noisy = ops.add_noise(latents, fwd_noise, t32, ac)
-        if u_encoder_hidden_states is not None and self.drop_prob is not None:      # train with classifier-free guidance (:539-543)
-            if drop_mask is None:
-                drop_mask = torch.bernoulli(torch.zeros(bsz) + self.drop_prob)       # drawn on the host, as the reference does (:541)
-            encoder_hidden_states = _CfgDropFn.apply(encoder_hidden_states, u_encoder_hidden_states.to(encoder_hidden_states.dtype),
-                                                     drop_mask.detach().to("cpu"))
-        cond = self.projector(encoder_hidden_states)[-1]
-        snr = None if self.snr_gamma is None else (ac, float(self.snr_gamma))
-        return _DiffusionLossFn.apply(cond, self.unet, noisy, t32, noise, snr)      # epsilon prediction (:548-549)
+        return noisy, noise, t32, ac
 
     @torch.no_grad()
     def pipeline(self, height: int | None = None, width: int | None = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
@@ -626,7 +640,16 @@ class StableDiffusionHead(MultimodalHead):
                  cross_attention_kwargs=None, guidance_rescale: float = 0.0, scheduler: str = "ddpm", use_cuda_graph: bool = True):
         """reference :672-850.  `scheduler="ddpm"` is what the reference runs (its training DDPMScheduler, :379/:833);
         `"ddim"` (eta 0) is BASELINE.json's C4 sampler."""
-        from .unet import DenoiseLoop
+        height, width, prompt_embeds, negative_prompt_embeds = self._pipeline_inputs(height, width, num_images_per_prompt, latents,
+                                                                                     prompt_embeds, negative_prompt_embeds, output_type)
+        cond = self.projector(prompt_embeds)[-1]
+        if guidance_scale > 1.0:
+            assert negative_prompt_embeds is not None, "When using classifier free guidance, `negative_prompt_embeds` must be provided by LLM."
+            cond = torch.cat([self.projector(negative_prompt_embeds)[-1], cond])
+        return self._sample(cond, None, height, width, num_inference_steps, guidance_scale, generator, latents, output_type, callback,
+                            callback_steps, guidance_rescale, scheduler, use_cuda_graph)
+
+    def _pipeline_inputs(self, height, width, num_images_per_prompt, latents, prompt_embeds, negative_prompt_embeds, output_type):
         height = height or self.resolution
         width = width or self.resolution
         if height % 8 or width % 8:
@@ -641,12 +664,13 @@ class StableDiffusionHead(MultimodalHead):
                 raise ValueError(f"latents batch {latents.shape[0]} != prompts x num_images_per_prompt = {prompt_embeds.shape[0]}")
         if output_type not in ("latent", "pt", "np", "pil"):
             raise ValueError(f"output_type must be one of 'latent', 'pt', 'np', 'pil', got {output_type!r}")
-        cond = self.projector(prompt_embeds)[-1]
-        if guidance_scale > 1.0:
-            assert negative_prompt_embeds is not None, "When using classifier free guidance, `negative_prompt_embeds` must be provided by LLM."
-            cond = torch.cat([self.projector(negative_prompt_embeds)[-1], cond])
+        return height, width, prompt_embeds, negative_prompt_embeds
+
+    def _sample(self, cond, aug_emb, height, width, num_inference_steps, guidance_scale, generator, latents, output_type, callback,
+                callback_steps, guidance_rescale, scheduler, use_cuda_graph):
+        from .unet import DenoiseLoop
         loop = DenoiseLoop(self.unet, cond, num_inference_steps, guidance_scale, scheduler, latents=latents, height=height, width=width,
-                           use_cuda_graph=use_cuda_graph, generator=generator, guidance_rescale=guidance_rescale)
+                           use_cuda_graph=use_cuda_graph, generator=generator, guidance_rescale=guidance_rescale, aug_emb=aug_emb)
         lat = loop.run(callback=callback, callback_steps=callback_steps)
         if output_type == "latent":
             return lat
@@ -656,3 +680,170 @@ class StableDiffusionHead(MultimodalHead):
             return image
         arr = image.permute(0, 2, 3, 1).cpu().numpy()
         return arr if output_type == "np" else numpy_to_pil(arr)
+
+
+# ------------------------------------------------------------------------------------------------ StableDiffusionXLHead
+class _MeanRowsFn(torch.autograd.Function):
+    """[B, Q, H] -> mean over Q, [B, H] (torch.mean of a bf16 tensor: fp32 accumulate, one rounding), on the channel-sum kernel."""
+
+    @staticmethod
+    def forward(ctx, x):
+        ctx.rows = x.shape[1]
+        return ops.mean_rows(x.contiguous())
+
+    @staticmethod
+    def backward(ctx, dy):
+        return ops.broadcast_rows(dy.contiguous(), ctx.rows, 1.0 / ctx.rows)
+
+
+class _DiffusionXLLossFn(torch.autograd.Function):
+    """`_DiffusionLossFn` for an SDXL UNet: the loss also depends on the pooled conditioning `text_embeds` through the addition
+    embedding, so the dgrad-only backward returns d(loss)/d(cond) and d(loss)/d(text_embeds)."""
+
+    @staticmethod
+    def forward(ctx, cond, text_embeds, unet, noisy, t32, target, time_ids, snr=None):
+        need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+
+        def mse(eps):
+            if snr is None:
+                return ops.mse_fwd_bwd(eps, target)
+            return ops.mse_minsnr_fwd_bwd(eps, target, t32, snr[0], snr[1])
+
+        with torch.no_grad():
+            eps, tape = unet.forward_train(noisy, t32, cond, (text_embeds, time_ids))
+            loss, deps = mse(eps)
+            if need:
+                dcond, dtext = unet.backward_cond(deps, tape)
+                ctx.save_for_backward(dcond.to(cond.dtype), dtext.to(text_embeds.dtype))
+            del tape
+        ctx.has_grad = need
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        if not ctx.has_grad:
+            return (None,) * 8
+        dcond, dtext = ctx.saved_tensors
+        return dcond * g.to(dcond.dtype), dtext * g.to(dtext.dtype), None, None, None, None, None, None
+
+
+def _check_scheduler_config(path):
+    """The sampler and the training noise use SD-2.1's DDPM tables (`unet.scheduler_tables`, `_alphas_cumprod`); SDXL-base's scheduler
+    folder has the same betas, spacing, offset and prediction type.  A config that differs is refused rather than sampled wrongly."""
+    import json
+    with open(path) as f:
+        cfg = json.load(f)
+    want = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear", prediction_type="epsilon",
+                steps_offset=1, timestep_spacing="leading")
+    bad = {k: cfg[k] for k, v in want.items() if k in cfg and cfg[k] != v}
+    if bad:
+        raise ValueError(f"{path}: {bad} differ from the supported scheduler {want}")
+
+
+class StableDiffusionXLHead(StableDiffusionHead):
+    """Mirror of reference `StableDiffusionXLHead` (omni/models/dreamllm_sdxl/modeling_plugins.py:47-445): the SD head on the SDXL UNet,
+    plus `global_projector`, which maps the mean of the dream-query states to SDXL's pooled `text_embeds` [B, 1280].
+
+    Training (:151-236): loss = mse(unet(noisy, t, projector(E), text_embeds=global_projector(mean_Q(E)), time_ids)); gradients reach E
+    through the cross-attention and through the time embedding of every resnet.  The reference has no CFG-dropout training for this
+    head (:202): `u_encoder_hidden_states` and `drop_prob` are ignored.  The VAE runs bf16 like the SD-2.1 head's (the reference keeps it
+    fp32); `processor` is None, as the base head's."""
+    _unet_config = SDXL
+    _vae_config = dict(scaling_factor=0.13025)
+
+    def __init__(self, diffusion_name_or_path=None, pretrained_model_name_or_path: str = None, projector_type="linear",
+                 projector_depth: int = 1, projector_name_or_path: str = None, embed_hidden_size: int = 4096,
+                 global_condition_hidden_size: int = 1280, drop_prob: float | None = None, noise_offset: float = 0.0,
+                 input_perturbation: float = 0.0, snr_gamma: float | None = None, resolution: int = 1024, center_crop: bool = True,
+                 random_flip: bool = True, freeze_vae: bool = True, freeze_unet: bool = True, freeze_projector: bool = False,
+                 local_files_only: bool = True):
+        if isinstance(diffusion_name_or_path, str):
+            sched = os.path.join(diffusion_name_or_path, "scheduler", "scheduler_config.json")
+            if os.path.isfile(sched):
+                _check_scheduler_config(sched)
+        super().__init__(diffusion_name_or_path=diffusion_name_or_path, projector_type=projector_type, projector_depth=projector_depth,
+                         projector_name_or_path=projector_name_or_path, pretrained_model_name_or_path=None,
+                         embed_hidden_size=embed_hidden_size, drop_prob=drop_prob, noise_offset=noise_offset,
+                         input_perturbation=input_perturbation, snr_gamma=snr_gamma, resolution=resolution, center_crop=center_crop,
+                         random_flip=random_flip, freeze_vae=freeze_vae, freeze_unet=freeze_unet, freeze_projector=freeze_projector,
+                         local_files_only=local_files_only)
+        if self.unet.add_embedding is None:
+            raise ValueError("StableDiffusionXLHead needs a UNet with addition_embed_type 'text_time'")
+        self.save_model_name = "stable_diffusion_xl_head"
+        self.pretrained_model_name_or_path = pretrained_model_name_or_path
+        self.global_condition_hidden_size = global_condition_hidden_size
+        projector_cfg = dict(projector=projector_type, freeze_projector=freeze_projector, depth=projector_depth,
+                             save_model_name=self.save_model_name, model_name_or_path=None)
+        # the reference's builder passes bias=None through; its projector classes default to a bias for "linear" and none for "mlp"
+        self.global_projector = build_projector(projector_cfg, in_hidden_size=embed_hidden_size, out_hidden_size=global_condition_hidden_size,
+                                                bias=projector_type == "linear")
+        if not self.global_projector.load_model(projector_name_or_path):
+            self._init_weights(self.global_projector)
+        if pretrained_model_name_or_path is not None:
+            self.load_model(pretrained_model_name_or_path)
+        self.global_projector.requires_grad_(not freeze_projector)
+
+    @property
+    def config(self):
+        return dict(diffusion_name_or_path=self.diffusion_name_or_path, pretrained_model_name_or_path=self.pretrained_model_name_or_path,
+                    embed_hidden_size=self.embed_hidden_size, global_condition_hidden_size=self.global_condition_hidden_size,
+                    drop_prob=self.drop_prob, noise_offset=self.noise_offset, input_perturbation=self.input_perturbation,
+                    snr_gamma=self.snr_gamma, freeze_vae=self.freeze_vae, freeze_unet=self.freeze_unet, freeze_projector=self.freeze_projector)
+
+    def fsdp_ignored_modules(self) -> list:
+        out = []
+        if self.freeze_vae:
+            out.append(self.vae)
+        if self.freeze_unet:
+            out.append(self.unet)
+        if self.freeze_projector:
+            out += [self.projector, self.global_projector]
+        return out
+
+    def text_embeds(self, encoder_hidden_states):
+        """Pooled conditioning [B, 1280] = global_projector(mean over the dream queries) (reference :197-199)."""
+        return self.global_projector(_MeanRowsFn.apply(encoder_hidden_states))[-1]
+
+    def forward(self, images=None, encoder_hidden_states=None, u_encoder_hidden_states=None, add_time_ids=None, dream_embeddings=None, *,
+                latents=None, noise=None, timesteps=None, vae_noise=None, offset_noise=None, perturbation_noise=None, drop_mask=None):
+        """Diffusion loss, reference :151-236.  add_time_ids [B, 6] = (original size, crop top-left, target size) per image, as the
+        data processor emits them.  The injectable draws are the base head's."""
+        if images is None and latents is None:
+            return None
+        if add_time_ids is None:
+            raise ValueError("StableDiffusionXLHead.forward needs add_time_ids [B, 6] (original_size + crops_coords_top_left + target_size)")
+        noisy, noise, t32, ac = self._noisy_latents(images, encoder_hidden_states, latents, noise, timesteps, vae_noise, offset_noise,
+                                                    perturbation_noise)
+        if tuple(add_time_ids.shape) != (noisy.shape[0], 6):
+            raise ValueError(f"add_time_ids must be [{noisy.shape[0]}, 6], got {tuple(add_time_ids.shape)}")
+        text = self.text_embeds(encoder_hidden_states)
+        cond = self.projector(encoder_hidden_states)[-1]
+        snr = None if self.snr_gamma is None else (ac, float(self.snr_gamma))
+        return _DiffusionXLLossFn.apply(cond, text, self.unet, noisy, t32, noise, add_time_ids.to(noisy.device), snr)
+
+    @torch.no_grad()
+    def pipeline(self, height: int | None = None, width: int | None = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
+                 num_images_per_prompt: int | None = 1, eta: float = 0.0, generator=None, latents=None, prompt_embeds=None,
+                 negative_prompt_embeds=None, output_type: str | None = "latent", callback=None, callback_steps: int = 1,
+                 cross_attention_kwargs=None, guidance_rescale: float = 0.0, scheduler: str = "ddpm", use_cuda_graph: bool = True,
+                 original_size=None, crops_coords_top_left=(0, 0), target_size=None):
+        """reference :238-445.  Time ids default to (1024, 1024, 0, 0, 1024, 1024) (sample_size 128 x the VAE's 8) in the prompt dtype;
+        the projectors also run on the negative prompt; aug_emb is computed once, outside the captured loop."""
+        height, width, prompt_embeds, negative_prompt_embeds = self._pipeline_inputs(height, width, num_images_per_prompt, latents,
+                                                                                     prompt_embeds, negative_prompt_embeds, output_type)
+        default = self.unet.cfg.get("sample_size", 128) * self.vae_scale_factor
+        original_size = tuple(original_size) if original_size is not None else (default, default)
+        target_size = tuple(target_size) if target_size is not None else original_size
+        ids = list(original_size) + list(crops_coords_top_left) + list(target_size)
+        B = prompt_embeds.shape[0]
+        time_ids = torch.tensor([ids], dtype=prompt_embeds.dtype, device=prompt_embeds.device).repeat(B, 1)
+        cond = self.projector(prompt_embeds)[-1]
+        text = self.text_embeds(prompt_embeds)
+        if guidance_scale > 1.0:
+            assert negative_prompt_embeds is not None, "When using classifier free guidance, `negative_prompt_embeds` must be provided by LLM."
+            cond = torch.cat([self.projector(negative_prompt_embeds)[-1], cond])
+            text = torch.cat([self.text_embeds(negative_prompt_embeds), text])
+            time_ids = torch.cat([time_ids, time_ids])
+        aug = self.unet.add_embedding_fwd(text, time_ids)
+        return self._sample(cond, aug, height, width, num_inference_steps, guidance_scale, generator, latents, output_type, callback,
+                            callback_steps, guidance_rescale, scheduler, use_cuda_graph)

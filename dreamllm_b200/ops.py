@@ -591,6 +591,16 @@ def col2im_s2(dcols2d, N, H, W, C):
     return dx
 
 
+def copy_cols_(src2d, dst2d, col0):
+    """dst2d[:, col0 : col0 + src cols] = src2d (both contiguous bf16, widths and col0 multiples of 8)."""
+    _chk_cuda(src2d, dst2d)
+    rows, Cs = src2d.shape
+    assert src2d.is_contiguous() and dst2d.is_contiguous() and dst2d.shape[0] == rows and col0 % 8 == 0 and col0 + Cs <= dst2d.shape[1]
+    check(lib().dllm_copy_cols(_p(src2d), _p(dst2d), rows, Cs, dst2d.shape[1], col0, _stream()), "dllm_copy_cols")
+    LAUNCHES.add(1)
+    return dst2d
+
+
 def split_channels(x_nhwc, c_first):
     """inverse of concat_channels: returns (x[..., :c_first], x[..., c_first:]) as contiguous tensors."""
     N, H, W, C = x_nhwc.shape
@@ -834,6 +844,72 @@ def attn_probs(q, k, lse, causal=True, seqlens=None, kv_len=None, kv_mask=None, 
                                     q.stride(1), k.stride(1), int(causal), scale, _stream()), "dllm_attn_probs_gqa")
     LAUNCHES.add(1)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ SDXL addition embedding
+def channel_sum_nhwc(x, out=None, *, scale=1.0, out_dtype=torch.float32):
+    """out[n, c] = scale * sum over the middle axes of x [N, ..., C] bf16 (fp32 accumulate, one rounding; deterministic).
+    `out` may be a [N, C] column slice of a wider buffer (unit inner stride); otherwise a new [N, C] tensor of `out_dtype`."""
+    _chk_cuda(x, out)
+    N, C = x.shape[0], x.shape[-1]
+    HW = x.numel() // (N * C)
+    assert x.dtype == BF16 and x.is_contiguous()
+    if out is None:
+        out = torch.empty((N, C), device=x.device, dtype=out_dtype)
+    assert out.shape == (N, C) and out.stride(1) == 1 and out.dtype in (BF16, torch.float32)
+    wsb = lib().dllm_channel_sum_workspace_bytes(N, HW, C)
+    ws = torch.empty(wsb, device=x.device, dtype=torch.uint8)
+    check(lib().dllm_channel_sum_nhwc(_p(x), _p(out), out.stride(0), int(out.dtype == BF16), float(scale), N, HW, C, _p(ws), wsb,
+                                      _stream()), "dllm_channel_sum_nhwc")
+    LAUNCHES.add(2)
+    return out
+
+
+def mean_rows(x):
+    """x [B, R, H] bf16 -> mean over R as bf16 [B, H] (fp32 accumulate, one rounding: torch.mean of a bf16 tensor)."""
+    return channel_sum_nhwc(x, scale=1.0 / x.shape[1], out_dtype=BF16)
+
+
+def broadcast_rows(src, R, scale=1.0):
+    """src [B, H] bf16 -> [B, R, H] with every row scale * src[b]."""
+    _chk_cuda(src)
+    B, H = src.shape
+    assert src.dtype == BF16 and src.is_contiguous()
+    out = torch.empty((B, R, H), device=src.device, dtype=BF16)
+    check(lib().dllm_broadcast_rows(_p(src), _p(out), B, R, H, float(scale), _stream()), "dllm_broadcast_rows")
+    LAUNCHES.add(1)
+    return out
+
+
+def time_ids_embedding(time_ids, out, dim=256):
+    """Timesteps(dim, flip_sin_to_cos=True, shift 0) of float ids [B, n] -> bf16 [cos | sin] per id, written into `out` [B, n * dim]
+    (a column slice of add_embeds is fine)."""
+    _chk_cuda(time_ids, out)
+    ids = time_ids.float().contiguous()
+    B, n = ids.shape
+    assert out.dtype == BF16 and out.shape == (B, n * dim) and out.stride(1) == 1
+    check(lib().dllm_time_ids_embedding(_p(ids), _p(out), out.stride(0), B, n, dim, _stream()), "dllm_time_ids_embedding")
+    LAUNCHES.add(1)
+    return out
+
+
+def silu(x):
+    _chk_cuda(x)
+    assert x.dtype == BF16 and x.is_contiguous()
+    y = torch.empty_like(x)
+    check(lib().dllm_silu_bf16(_p(x), _p(y), x.numel(), _stream()), "dllm_silu_bf16")
+    LAUNCHES.add(1)
+    return y
+
+
+def silu_bwd(dy, x):
+    """dx = dy * silu'(x)."""
+    _chk_cuda(dy, x)
+    assert dy.dtype == x.dtype == BF16 and dy.is_contiguous() and x.is_contiguous() and dy.shape == x.shape
+    dx = torch.empty_like(x)
+    check(lib().dllm_silu_bwd_bf16(_p(dy), _p(x), _p(dx), x.numel(), _stream()), "dllm_silu_bwd_bf16")
+    LAUNCHES.add(1)
+    return dx
 
 
 # ------------------------------------------------------------------------------------------------ optimizer shard (SURVEY §8f row 4)

@@ -30,6 +30,13 @@ BF16 = torch.bfloat16
 SD21 = dict(in_channels=4, out_channels=4, block_out_channels=(320, 640, 1280, 1280), layers_per_block=2,
             attention_head_dim=(5, 10, 20, 20), cross_attention_dim=1024, norm_num_groups=32, norm_eps=1e-5,
             down_attn=(True, True, True, False), up_attn=(False, True, True, True))
+# SDXL-base unet/config.json (diffusers 0.24): no attention at the 320 level, transformer depth 1 / 2 / 10 (the mid block takes the last,
+# the up blocks the reversed list), and the "text_time" addition embedding: add_embedding(cat(text_embeds [B, 1280],
+# Timesteps(256)(time_ids [B, 6]))) is added to the time embedding.  2 567 463 684 parameters.
+SDXL = dict(in_channels=4, out_channels=4, block_out_channels=(320, 640, 1280), layers_per_block=2, attention_head_dim=(5, 10, 20),
+            cross_attention_dim=2048, norm_num_groups=32, norm_eps=1e-5, down_attn=(False, True, True), up_attn=(True, True, False),
+            transformer_layers_per_block=(1, 2, 10), addition_embed_type="text_time", addition_time_embed_dim=256,
+            projection_class_embeddings_input_dim=2816)
 
 
 # ------------------------------------------------------------------------------------------------ parameter containers
@@ -86,11 +93,11 @@ class BasicTransformerBlock(nn.Module):
 
 
 class Transformer2DModel(nn.Module):
-    def __init__(self, dim, heads, ctx_dim, groups):
+    def __init__(self, dim, heads, ctx_dim, groups, depth=1):
         super().__init__()
         self.norm = nn.GroupNorm(groups, dim, eps=1e-6)
         self.proj_in = nn.Linear(dim, dim)
-        self.transformer_blocks = nn.ModuleList([BasicTransformerBlock(dim, heads, ctx_dim)])
+        self.transformer_blocks = nn.ModuleList([BasicTransformerBlock(dim, heads, ctx_dim) for _ in range(depth)])
         self.proj_out = nn.Linear(dim, dim)
 
 
@@ -120,10 +127,20 @@ class UNet2DConditionModel(nn.Module):
                                     c["layers_per_block"], c["norm_eps"])
         for co, h in zip(ch, heads):
             if co // h != 64:
-                raise ValueError("UNet attention head_dim must be 64 (SD-2.x)")
+                raise ValueError(f"UNet attention head_dim must be 64 (block_out_channels {tuple(ch)} / attention_head_dim {tuple(heads)} "
+                                 f"gives {co} / {h}); SD-2.x and SDXL both use 64")
+        depth = tuple(c.get("transformer_layers_per_block") or (1,) * len(ch))
+        if len(depth) != len(ch):
+            raise ValueError(f"transformer_layers_per_block {depth} needs one entry per level ({len(ch)})")
+        add_type = c.get("addition_embed_type")
+        if add_type not in (None, "text_time"):
+            raise ValueError(f"addition_embed_type {add_type!r} is not built (None or 'text_time')")
         temb = ch[0] * 4
         self.conv_in = nn.Conv2d(c["in_channels"], ch[0], 3, padding=1)
         self.time_embedding = TimestepEmbedding(ch[0], temb)
+        self.add_embedding = None
+        if add_type == "text_time":
+            self.add_embedding = TimestepEmbedding(c["projection_class_embeddings_input_dim"], temb)
         self.down_blocks = nn.ModuleList()
         out = ch[0]
         for i, co in enumerate(ch):
@@ -131,15 +148,15 @@ class UNet2DConditionModel(nn.Module):
             cin, out = out, co
             b.resnets = nn.ModuleList([ResnetBlock2D(cin if j == 0 else out, out, temb, G, eps) for j in range(L)])
             if c["down_attn"][i]:
-                b.attentions = nn.ModuleList([Transformer2DModel(out, heads[i], ctx, G) for _ in range(L)])
+                b.attentions = nn.ModuleList([Transformer2DModel(out, heads[i], ctx, G, depth[i]) for _ in range(L)])
             if i < len(ch) - 1:
                 b.downsamplers = nn.ModuleList([Downsample2D(out)])
             self.down_blocks.append(b)
         self.mid_block = _Block()
         self.mid_block.resnets = nn.ModuleList([ResnetBlock2D(ch[-1], ch[-1], temb, G, eps), ResnetBlock2D(ch[-1], ch[-1], temb, G, eps)])
-        self.mid_block.attentions = nn.ModuleList([Transformer2DModel(ch[-1], heads[-1], ctx, G)])
+        self.mid_block.attentions = nn.ModuleList([Transformer2DModel(ch[-1], heads[-1], ctx, G, depth[-1])])
         self.up_blocks = nn.ModuleList()
-        rev, rheads = list(reversed(ch)), list(reversed(heads))
+        rev, rheads, rdepth = list(reversed(ch)), list(reversed(heads)), list(reversed(depth))
         prev = rev[0]
         for i, co in enumerate(rev):
             b = _Block()
@@ -147,7 +164,7 @@ class UNet2DConditionModel(nn.Module):
             b.resnets = nn.ModuleList([ResnetBlock2D((prev if j == 0 else co) + (skip_in if j == L else co), co, temb, G, eps)
                                        for j in range(L + 1)])
             if c["up_attn"][i]:
-                b.attentions = nn.ModuleList([Transformer2DModel(co, rheads[i], ctx, G) for _ in range(L + 1)])
+                b.attentions = nn.ModuleList([Transformer2DModel(co, rheads[i], ctx, G, rdepth[i]) for _ in range(L + 1)])
             if i < len(ch) - 1:
                 b.upsamplers = nn.ModuleList([Upsample2D(co)])
             prev = co
@@ -174,6 +191,56 @@ class UNet2DConditionModel(nn.Module):
                 for t in b.attentions:
                     yield t
 
+    def blocks(self):
+        """Every BasicTransformerBlock in forward order (16 for SD-2.1, 70 for SDXL): one cross-attention K/V tensor each."""
+        for t in self.transformers():
+            yield from t.transformer_blocks
+
+    def resnets(self):
+        """Every ResnetBlock2D in forward order."""
+        for b in self.down_blocks:
+            yield from b.resnets
+        yield from self.mid_block.resnets
+        for b in self.up_blocks:
+            yield from b.resnets
+
+    # ---- addition embedding (SDXL "text_time") ----
+    def _add_embedding(self, text_embeds, time_ids):
+        """aug_emb = add_embedding(cat(text_embeds, Timesteps(256)(time_ids))) as diffusers computes it (the sinusoid in fp32, the
+        concatenation rounded once to bf16).  Returns (add_embeds, pre-SiLU linear_1 output, aug_emb), all bf16 [B, *]."""
+        ae = self.add_embedding
+        B, ct = text_embeds.shape
+        n_ids = time_ids.shape[-1]
+        dim = self.cfg["addition_time_embed_dim"]
+        if ae.linear_1.weight.shape[1] != ct + n_ids * dim:
+            raise ValueError(f"text_embeds [{B}, {ct}] + time_ids [{B}, {n_ids}] x {dim} != projection_class_embeddings_input_dim "
+                             f"{ae.linear_1.weight.shape[1]}")
+        add = torch.empty((B, ct + n_ids * dim), device=text_embeds.device, dtype=BF16)
+        ops.copy_cols_(text_embeds.to(BF16).contiguous(), add, 0)
+        ops.time_ids_embedding(time_ids.reshape(B, n_ids), add[:, ct:], dim)
+        z1 = ops.linear(add, ae.linear_1.weight, bias=ae.linear_1.bias)
+        aug = ops.linear(ops.silu(z1), ae.linear_2.weight, bias=ae.linear_2.bias)
+        return add, z1, aug
+
+    @torch.no_grad()
+    def add_embedding_fwd(self, text_embeds, time_ids):
+        """SDXL's per-prompt aug_emb [B, 1280] (timestep-invariant: computed once per `pipeline` call, outside the sampler graph)."""
+        if self.add_embedding is None:
+            raise ValueError("this UNet has no addition embedding (addition_embed_type is None)")
+        return self._add_embedding(text_embeds, time_ids)[2]
+
+    def _temb_act(self, temb_sin, aug_emb):
+        """silu(time_embedding(t) [+ aug_emb]): the activation every resnet's time_emb_proj reads.  With aug_emb the sum is rounded to
+        bf16 before the SiLU (diffusers: emb = emb + aug_emb, then silu in each resnet); returns (temb or None, silu(temb))."""
+        te = self.time_embedding
+        if (aug_emb is None) != (self.add_embedding is None):
+            raise ValueError("an SDXL UNet (addition_embed_type 'text_time') needs text_embeds / time_ids and an SD-2.x UNet takes none")
+        t1 = ops.linear(temb_sin, te.linear_1.weight, bias=te.linear_1.bias, act=ops.ACT_SILU)
+        if aug_emb is None:
+            return None, ops.linear(t1, te.linear_2.weight, bias=te.linear_2.bias, act=ops.ACT_SILU)
+        temb = ops.linear(t1, te.linear_2.weight, bias=te.linear_2.bias, residual=aug_emb)     # the epilogue adds residual after act
+        return temb, ops.silu(temb)
+
     # ---- building blocks (x: NHWC bf16) ----
     def _resnet(self, r: ResnetBlock2D, x, temb_act):
         N, H, W, Cin = x.shape
@@ -189,14 +256,20 @@ class UNet2DConditionModel(nn.Module):
             sc = ops.linear(x.view(-1, Cin), wsc, bias=r.conv_shortcut.bias).view(N, H, W, -1)
         return ops.conv3x3(h, self._conv_w(r.conv2), bias=r.conv2.bias, residual=sc)
 
-    def _transformer(self, t: Transformer2DModel, x, ctx_kv):
+    def _transformer(self, t: Transformer2DModel, x, kv):
+        """kv: iterator over the per-block cross K/V tensors of `precompute_cross_kv` (one per BasicTransformerBlock)."""
         N, H, W, C = x.shape
-        T, S = N * H * W, H * W
-        blk = t.transformer_blocks[0]
-        nh = blk.attn1.heads
+        T = N * H * W
         x2 = x.view(T, C)
         h = ops.groupnorm(x, t.norm.weight, t.norm.bias, self.cfg["norm_num_groups"], t.norm.eps, silu=False).view(T, C)
         h = ops.linear(h, t.proj_in.weight, bias=t.proj_in.bias)
+        for blk in t.transformer_blocks:
+            h = self._block(blk, h, next(kv), N, H * W)
+        return ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
+
+    def _block(self, blk: BasicTransformerBlock, h, ctx_kv, N, S):
+        T, C = h.shape
+        nh = blk.attn1.heads
         # self-attention
         y = ops.layernorm_fwd(h, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
         wqkv = _fuse_rows([blk.attn1.to_q.weight, blk.attn1.to_k.weight, blk.attn1.to_v.weight])
@@ -213,8 +286,7 @@ class UNet2DConditionModel(nn.Module):
         # GEGLU feed-forward
         y = ops.layernorm_fwd(h, blk.norm3.weight, blk.norm3.bias, blk.norm3.eps)
         g = ops.linear_geglu(y, *self._geglu_w(blk.ff.net[0].proj))       # FF-in GEMM with h * gelu(gate) in its epilogue
-        h = ops.linear(g, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h)
-        return ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
+        return ops.linear(g, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h)
 
     def _geglu_w(self, proj: nn.Linear):
         """Row-permuted copy of `GEGLU.proj` ([64 value | 64 gate] per 128 rows) for the fused epilogue; the parameter itself keeps the
@@ -233,19 +305,17 @@ class UNet2DConditionModel(nn.Module):
         N, Q, D = encoder_hidden_states.shape
         e2 = encoder_hidden_states.to(BF16).reshape(N * Q, D).contiguous()
         out = []
-        for t in self.transformers():
-            a = t.transformer_blocks[0].attn2
+        for blk in self.blocks():
+            a = blk.attn2
             wkv = _fuse_rows([a.to_k.weight, a.to_v.weight])
             out.append(ops.linear(e2, wkv).view(N, Q, -1))
         return out
 
     @torch.no_grad()
-    def forward_nhwc(self, latents_nchw_f32, temb_sin, cross_kv, batch, eps_out=None):
+    def forward_nhwc(self, latents_nchw_f32, temb_sin, cross_kv, batch, eps_out=None, aug_emb=None):
         """latents [Bl,4,H,W] fp32 (Bl divides batch: CFG duplication); temb_sin [batch, 320] bf16 sinusoidal embedding;
-        cross_kv from `precompute_cross_kv` -> eps [batch,4,H,W] fp32."""
-        te = self.time_embedding
-        t1 = ops.linear(temb_sin, te.linear_1.weight, bias=te.linear_1.bias, act=ops.ACT_SILU)
-        temb_act = ops.linear(t1, te.linear_2.weight, bias=te.linear_2.bias, act=ops.ACT_SILU)    # silu(temb): all the resnets read
+        cross_kv from `precompute_cross_kv`; aug_emb [batch, 1280] bf16 from `add_embedding_fwd` (SDXL only) -> eps [batch,4,H,W] fp32."""
+        _, temb_act = self._temb_act(temb_sin, aug_emb)          # silu(temb): all the resnets read
         x = ops.conv_in(latents_nchw_f32, self.conv_in.weight, self.conv_in.bias, batch)
         skips = [x]
         kv = iter(cross_kv)
@@ -253,7 +323,7 @@ class UNet2DConditionModel(nn.Module):
             for j, r in enumerate(b.resnets):
                 x = self._resnet(r, x, temb_act)
                 if hasattr(b, "attentions"):
-                    x = self._transformer(b.attentions[j], x, next(kv))
+                    x = self._transformer(b.attentions[j], x, kv)
                 skips.append(x)
             if hasattr(b, "downsamplers"):
                 conv = b.downsamplers[0].conv
@@ -262,13 +332,13 @@ class UNet2DConditionModel(nn.Module):
                 x = ops.linear(cols, self._conv_w(conv), bias=conv.bias).view(N, H // 2, W // 2, -1)
                 skips.append(x)
         x = self._resnet(self.mid_block.resnets[0], x, temb_act)
-        x = self._transformer(self.mid_block.attentions[0], x, next(kv))
+        x = self._transformer(self.mid_block.attentions[0], x, kv)
         x = self._resnet(self.mid_block.resnets[1], x, temb_act)
         for b in self.up_blocks:
             for j, r in enumerate(b.resnets):
                 x = self._resnet(r, ops.concat_channels(x, skips.pop()), temb_act)
                 if hasattr(b, "attentions"):
-                    x = self._transformer(b.attentions[j], x, next(kv))
+                    x = self._transformer(b.attentions[j], x, kv)
             if hasattr(b, "upsamplers"):
                 conv = b.upsamplers[0].conv
                 x = ops.conv3x3(ops.upsample2x(x), self._conv_w(conv), bias=conv.bias)
@@ -307,12 +377,16 @@ class UNet2DConditionModel(nn.Module):
         tape.append(("res", r, x, st1, c1, st2))
         return out
 
-    def _resnet_bwd(self, ent, dout):
+    def _resnet_bwd(self, ent, dout, drowb=None):
+        """drowb: {resnet: [N, Cout] bf16 column slice} when the time embedding needs a gradient (SDXL); the resnet's time_emb_proj
+        output gradient, sum over pixels of d(conv1 output), is written there."""
         _, r, x, st1, c1, st2 = ent
         N, H, W, Cin = x.shape
         G = self.cfg["norm_num_groups"]
         dh2 = ops.conv3x3(dout, self._conv_w_dgrad(r.conv2))
         dc1 = ops.groupnorm_bwd(dh2, c1, r.norm2.weight, r.norm2.bias, st2, G, True)
+        if drowb is not None:
+            ops.channel_sum_nhwc(dc1, out=drowb[r])
         dh1 = ops.conv3x3(dc1, self._conv_w_dgrad(r.conv1))
         if r.conv_shortcut is None:
             dsc = dout
@@ -321,14 +395,22 @@ class UNet2DConditionModel(nn.Module):
             dsc = ops.linear_dgrad(dout.view(-1, Cout), r.conv_shortcut.weight.view(Cout, Cin)).view(N, H, W, Cin)
         return ops.groupnorm_bwd(dh1, x, r.norm1.weight, r.norm1.bias, st1, G, True, dres=dsc)
 
-    def _transformer_fwd(self, t, x, ctx_kv, tape):
+    def _transformer_fwd(self, t, x, kv, tape):
         N, H, W, C = x.shape
         T, S = N * H * W, H * W
-        blk = t.transformer_blocks[0]
-        nh = blk.attn1.heads
         x2 = x.view(T, C)
         g, st = ops.groupnorm(x, t.norm.weight, t.norm.bias, self.cfg["norm_num_groups"], t.norm.eps, silu=False, return_stats=True)
-        h0 = ops.linear(g.view(T, C), t.proj_in.weight, bias=t.proj_in.bias)
+        h = ops.linear(g.view(T, C), t.proj_in.weight, bias=t.proj_in.bias)
+        saved = []
+        for blk in t.transformer_blocks:
+            h = self._block_fwd(blk, h, next(kv), N, S, saved)
+        out = ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
+        tape.append(("tr", t, x, st, saved))
+        return out
+
+    def _block_fwd(self, blk, h0, ctx_kv, N, S, saved):
+        T, C = h0.shape
+        nh = blk.attn1.heads
         y = ops.layernorm_fwd(h0, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
         wqkv = _fuse_rows([blk.attn1.to_q.weight, blk.attn1.to_k.weight, blk.attn1.to_v.weight])
         qkv = ops.linear(y, wqkv).view(N, S, 3, nh, 64)
@@ -344,18 +426,23 @@ class UNet2DConditionModel(nn.Module):
         f = ops.linear(y, blk.ff.net[0].proj.weight, bias=blk.ff.net[0].proj.bias)
         gg = ops.geglu(f)
         h3 = ops.linear(gg, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h2)
-        out = ops.linear(h3, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
-        tape.append(("tr", t, x, st, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f))
-        return out
+        saved.append((blk, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f))
+        return h3
 
     def _transformer_bwd(self, ent, dout, dkv_list):
-        _, t, x, st, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f = ent
+        _, t, x, st, saved = ent
         N, H, W, C = x.shape
         T, S = N * H * W, H * W
-        blk = t.transformer_blocks[0]
+        dh = ops.linear_dgrad(dout.view(T, C), t.proj_out.weight)
+        for sv in reversed(saved):
+            dh = self._block_bwd(sv, dh, N, S, dkv_list)
+        dg = ops.linear_dgrad(dh, t.proj_in.weight).view(N, H, W, C)
+        return ops.groupnorm_bwd(dg, x, t.norm.weight, t.norm.bias, st, self.cfg["norm_num_groups"], False, dres=dout)
+
+    def _block_bwd(self, sv, dh3, N, S, dkv_list):
+        blk, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f = sv
+        T, C = h0.shape
         nh = blk.attn1.heads
-        d2 = dout.view(T, C)
-        dh3 = ops.linear_dgrad(d2, t.proj_out.weight)
         # feed-forward
         dgg = ops.linear_dgrad(dh3, blk.ff.net[2].weight)
         df = ops.geglu_bwd(dgg, f)
@@ -369,7 +456,7 @@ class UNet2DConditionModel(nn.Module):
         dkv = torch.empty_like(ctx_kv)
         dkv5 = dkv.view(N, Q, 2, nh, 64)
         ops.attn_bwd_cross(dao2.view(N, S, C), q2, kv[:, :, 0], kv[:, :, 1], ao2, lse2, dq2, dkv5[:, :, 0], dkv5[:, :, 1])
-        dkv_list.append((t, dkv))
+        dkv_list.append((blk, dkv))
         dy = ops.linear_dgrad(dq2.view(T, C), blk.attn2.to_q.weight)
         dh1 = ops.layernorm_bwd(dy, h1, blk.norm2.weight, blk.norm2.eps, dres=dh2)
         # self-attention
@@ -379,24 +466,32 @@ class UNet2DConditionModel(nn.Module):
                      causal=False)
         wqkv = _fuse_rows([blk.attn1.to_q.weight, blk.attn1.to_k.weight, blk.attn1.to_v.weight])
         dy = ops.linear_dgrad(dqkv.view(T, 3 * C), wqkv)
-        dh0 = ops.layernorm_bwd(dy, h0, blk.norm1.weight, blk.norm1.eps, dres=dh1)
-        dg = ops.linear_dgrad(dh0, t.proj_in.weight).view(N, H, W, C)
-        return ops.groupnorm_bwd(dg, x, t.norm.weight, t.norm.bias, st, self.cfg["norm_num_groups"], False, dres=dout)
+        return ops.layernorm_bwd(dy, h0, blk.norm1.weight, blk.norm1.eps, dres=dh1)
 
-    def forward_train(self, latents_nchw_f32, t_i32, encoder_hidden_states):
-        """noisy latents [B,4,H,W] fp32, per-sample timesteps int32 [B], cond [B,Q,ctx] -> (eps [B,4,H,W] fp32, tape)."""
+    def forward_train(self, latents_nchw_f32, t_i32, encoder_hidden_states, added_cond=None):
+        """noisy latents [B,4,H,W] fp32, per-sample timesteps int32 [B], cond [B,Q,ctx] -> (eps [B,4,H,W] fp32, tape).
+        added_cond = (text_embeds [B, 1280], time_ids [B, 6]) for an SDXL UNet: the tape then also keeps what the gradient into
+        text_embeds (through add_embedding and every resnet's time_emb_proj) needs."""
         B = latents_nchw_f32.shape[0]
         tape = []
         cond2 = encoder_hidden_states.to(BF16).reshape(-1, encoder_hidden_states.shape[-1]).contiguous()
         Q = encoder_hidden_states.shape[1]
         kvs = []
-        for t in self.transformers():
-            a = t.transformer_blocks[0].attn2
+        for blk in self.blocks():
+            a = blk.attn2
             kvs.append(ops.linear(cond2, _fuse_rows([a.to_k.weight, a.to_v.weight])).view(B, Q, -1))
-        te = self.time_embedding
         temb_sin = ops.timestep_embedding_batch(t_i32, self.cfg["block_out_channels"][0])
-        t1 = ops.linear(temb_sin, te.linear_1.weight, bias=te.linear_1.bias, act=ops.ACT_SILU)
-        temb_act = ops.linear(t1, te.linear_2.weight, bias=te.linear_2.bias, act=ops.ACT_SILU)
+        xl = None
+        aug = None
+        if added_cond is not None:
+            if self.add_embedding is None:
+                raise ValueError("added_cond given to a UNet without an addition embedding (addition_embed_type is None)")
+            text_embeds, time_ids = added_cond
+            _, z1, aug = self._add_embedding(text_embeds, time_ids)
+            xl = dict(z1=z1, ct=text_embeds.shape[1])
+        temb, temb_act = self._temb_act(temb_sin, aug)
+        if xl is not None:
+            xl["temb"] = temb
         x = ops.conv_in(latents_nchw_f32, self.conv_in.weight, self.conv_in.bias, B)
         skips = [x]
         kv = iter(kvs)
@@ -404,7 +499,7 @@ class UNet2DConditionModel(nn.Module):
             for j, r in enumerate(b.resnets):
                 x = self._resnet_fwd(r, x, temb_act, tape)
                 if hasattr(b, "attentions"):
-                    x = self._transformer_fwd(b.attentions[j], x, next(kv), tape)
+                    x = self._transformer_fwd(b.attentions[j], x, kv, tape)
                 skips.append(x)
                 tape.append(("skip_push",))
             if hasattr(b, "downsamplers"):
@@ -415,7 +510,7 @@ class UNet2DConditionModel(nn.Module):
                 skips.append(x)
                 tape.append(("skip_push",))
         x = self._resnet_fwd(self.mid_block.resnets[0], x, temb_act, tape)
-        x = self._transformer_fwd(self.mid_block.attentions[0], x, next(kv), tape)
+        x = self._transformer_fwd(self.mid_block.attentions[0], x, kv, tape)
         x = self._resnet_fwd(self.mid_block.resnets[1], x, temb_act, tape)
         for b in self.up_blocks:
             for j, r in enumerate(b.resnets):
@@ -423,7 +518,7 @@ class UNet2DConditionModel(nn.Module):
                 tape.append(("cat", x.shape[-1]))
                 x = self._resnet_fwd(r, ops.concat_channels(x, sk), temb_act, tape)
                 if hasattr(b, "attentions"):
-                    x = self._transformer_fwd(b.attentions[j], x, next(kv), tape)
+                    x = self._transformer_fwd(b.attentions[j], x, kv, tape)
             if hasattr(b, "upsamplers"):
                 conv = b.upsamplers[0].conv
                 x = ops.conv3x3(ops.upsample2x(x), self._conv_w(conv), bias=conv.bias)
@@ -432,13 +527,24 @@ class UNet2DConditionModel(nn.Module):
                                silu=True, return_stats=True)
         tape.append(("out", x, stn))
         eps = ops.conv_out(xn, self.conv_out.weight, self.conv_out.bias)
-        return eps, (tape, B, Q)
+        return eps, (tape, B, Q, xl)
 
     def backward_cond(self, deps_nchw_f32, tape_pack):
-        """d(loss)/d(eps) [B,4,H,W] fp32 -> d(loss)/d(encoder_hidden_states) [B,Q,ctx] bf16."""
-        tape, B, Q = tape_pack
+        """d(loss)/d(eps) [B,4,H,W] fp32 -> d(loss)/d(encoder_hidden_states) [B,Q,ctx] bf16; for a tape recorded with `added_cond`,
+        (that, d(loss)/d(text_embeds) [B, 1280] bf16)."""
+        tape, B, Q, xl = tape_pack
         dkv_list = []
         skip_grads = []          # gradients flowing into skip connections, LIFO mirror of the forward's stack
+        drowb = None
+        if xl is not None:
+            # every resnet's time_emb_proj output gradient, side by side: one [B, sum Cout] operand for a single dgrad GEMM at the end
+            res = list(self.resnets())
+            drowb_all = torch.empty((B, sum(r.time_emb_proj.weight.shape[0] for r in res)), device=deps_nchw_f32.device, dtype=BF16)
+            drowb, col = {}, 0
+            for r in res:
+                co = r.time_emb_proj.weight.shape[0]
+                drowb[r] = drowb_all[:, col:col + co]
+                col += co
         ent = tape[-1]
         _, x_last, stn = ent
         C0 = x_last.shape[-1]
@@ -447,7 +553,7 @@ class UNet2DConditionModel(nn.Module):
         for ent in reversed(tape[:-1]):
             kind = ent[0]
             if kind == "res":
-                dx = self._resnet_bwd(ent, dx)
+                dx = self._resnet_bwd(ent, dx, drowb)
             elif kind == "tr":
                 dx = self._transformer_bwd(ent, dx, dkv_list)
             elif kind == "up":
@@ -466,25 +572,38 @@ class UNet2DConditionModel(nn.Module):
             else:
                 raise RuntimeError(kind)
         # conv_in's skip (the first push) has no upstream consumer of dx: the latents need no gradient
-        # cond gradient: sum over the 16 cross-attention blocks of dkv @ [Wk; Wv]
+        # cond gradient: sum over the cross-attention blocks (16 for SD-2.1, 70 for SDXL) of dkv @ [Wk; Wv]
         dcond = None
-        for t, dkv in dkv_list:
-            a = t.transformer_blocks[0].attn2
+        for blk, dkv in dkv_list:
+            a = blk.attn2
             g = ops.linear_dgrad(dkv.view(B * Q, -1), _fuse_rows([a.to_k.weight, a.to_v.weight]))
             dcond = g if dcond is None else ops.add(dcond, g)
-        return dcond.view(B, Q, -1)
+        dcond = dcond.view(B, Q, -1)
+        if xl is None:
+            return dcond
+        # text_embeds gradient: temb_act feeds every resnet's time_emb_proj, temb = time_embedding(t) + add_embedding(add_embeds)
+        w_temb = _fuse_rows([r.time_emb_proj.weight for r in self.resnets()])          # [sum Cout, 1280]
+        dtemb = ops.silu_bwd(ops.linear_dgrad(drowb_all, w_temb), xl["temb"])
+        ae = self.add_embedding
+        dz1 = ops.silu_bwd(ops.linear_dgrad(dtemb, ae.linear_2.weight), xl["z1"])
+        dtext = ops.linear_dgrad(dz1, ae.linear_1.weight[:, :xl["ct"]])              # only the text_embeds columns of add_embeds
+        return dcond, dtext
 
     @torch.no_grad()
-    def forward(self, sample, timestep, encoder_hidden_states):
-        """diffusers-style entry: sample [B,4,H,W], timestep int / tensor, encoder_hidden_states [B,Q,ctx] -> eps [B,4,H,W] fp32."""
+    def forward(self, sample, timestep, encoder_hidden_states, added_cond_kwargs=None):
+        """diffusers-style entry: sample [B,4,H,W], timestep int / tensor, encoder_hidden_states [B,Q,ctx] -> eps [B,4,H,W] fp32.
+        An SDXL UNet also takes added_cond_kwargs = {"text_embeds": [B, 1280], "time_ids": [B, 6]}."""
         if not sample.is_cuda:
             raise RuntimeError("dreamllm_b200 UNet requires CUDA tensors; there is no CPU fallback")
         B = sample.shape[0]
         dev = sample.device
+        aug = None
+        if added_cond_kwargs is not None:
+            aug = self.add_embedding_fwd(added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"])
         ts = torch.as_tensor(timestep, device=dev).reshape(-1)[:1].to(torch.int32)
         step0 = torch.zeros(1, device=dev, dtype=torch.int32)
         temb_sin = ops.timestep_embedding(ts, step0, B, self.cfg["block_out_channels"][0])
-        return self.forward_nhwc(sample.float().contiguous(), temb_sin, self.precompute_cross_kv(encoder_hidden_states), B)
+        return self.forward_nhwc(sample.float().contiguous(), temb_sin, self.precompute_cross_kv(encoder_hidden_states), B, aug_emb=aug)
 
 
 # ------------------------------------------------------------------------------------------------ sampler
@@ -535,9 +654,10 @@ class DenoiseLoop:
 
     def __init__(self, unet: UNet2DConditionModel, cond, num_inference_steps=50, guidance_scale=7.5, scheduler="ddim",
                  latents=None, noise=None, height=512, width=512, use_cuda_graph=True, generator=None, guidance_rescale: float = 0.0,
-                 whole_loop_graph: bool = True):
+                 whole_loop_graph: bool = True, aug_emb=None):
         """cond: [B, Q, ctx] projected prompt embeddings, or [2B, Q, ctx] = cat([negative, positive]) when guidance_scale > 1
-        (reference order, modeling_plugins.py:774-784)."""
+        (reference order, modeling_plugins.py:774-784).  aug_emb: an SDXL UNet's per-prompt addition embedding [B or 2B, 1280] bf16
+        (`UNet2DConditionModel.add_embedding_fwd`, same order as cond), added to the time embedding at every step."""
         self.unet = unet
         dev = cond.device
         self.use_cfg = guidance_scale > 1.0
@@ -560,6 +680,9 @@ class DenoiseLoop:
             self.noise = (torch.randn((self.N,) + tuple(self.latents.shape), generator=generator, device=dev) if noise is None
                           else noise.to(dev)).float().contiguous()
         self.cross_kv = unet.precompute_cross_kv(cond)
+        if aug_emb is not None and tuple(aug_emb.shape[:1]) != (self.nb,):
+            raise ValueError(f"aug_emb has {aug_emb.shape[0]} rows, cond has {self.nb}")
+        self.aug_emb = None if aug_emb is None else aug_emb.to(BF16).contiguous()
         self.eps = torch.empty((self.nb, 4, h, w), device=dev, dtype=torch.float32)
         self.graph = None              # single-step graph (callback path)
         self.loop_graph = None         # all N steps in one graph
@@ -591,7 +714,7 @@ class DenoiseLoop:
 
     def _one_step(self):
         temb_sin = ops.timestep_embedding(self.timesteps, self.step, self.nb, self.unet.cfg["block_out_channels"][0])
-        self.unet.forward_nhwc(self.latents, temb_sin, self.cross_kv, self.nb, eps_out=self.eps)
+        self.unet.forward_nhwc(self.latents, temb_sin, self.cross_kv, self.nb, eps_out=self.eps, aug_emb=self.aug_emb)
         if self.use_cfg and self.guidance_rescale > 0.0:          # (:826-831) guided prediction rescaled before the scheduler update
             eu, ec = self.eps[: self.B], self.eps[self.B:]
             self.eps[: self.B].copy_(rescale_noise_cfg(eu + self.guidance * (ec - eu), ec, self.guidance_rescale))

@@ -252,6 +252,25 @@ int dllm_adamw_step(const void* grad, void* master, void* exp_avg, void* exp_avg
 size_t dllm_sumsq_workspace_bytes(void);
 int dllm_sumsq_bf16(const void* x, long n, float* out, int accumulate, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- SDXL UNet addition embedding (diffusers UNet2DConditionModel, addition_embed_type "text_time") and the gradient that reaches the
+ * pooled conditioning through it: omni/models/dreamllm_sdxl/modeling_plugins.py:197-215 (global_projector(mean(1)), unet(...,
+ * added_cond_kwargs)), :344-395 (pipeline). ----
+ * out[n, c] = scale * sum_{hw < HW} x[n, hw, c] for x [N, HW, C] bf16 (C % 8 == 0), fp32 accumulate, written as fp32 (out_bf16 = 0) or
+ * bf16 into row n of out (row stride ldo >= C elements: a column slice of a wider buffer).  Deterministic: per-CTA partials, then a
+ * fixed-order pass, no atomics.  Used for each resnet's time_emb_proj bias gradient (sum over pixels of the conv1 output gradient)
+ * and for the mean over the dream queries (scale = 1/Q, bf16: torch.mean's single rounding). */
+size_t dllm_channel_sum_workspace_bytes(int N, int HW, int C);
+int dllm_channel_sum_nhwc(const void* x, void* out, long ldo, int out_bf16, float scale, int N, int HW, int C, void* workspace,
+                          size_t workspace_bytes, void* stream);
+/* Timesteps(dim, flip_sin_to_cos=True, shift 0) of fp32 ids [B, n_ids] -> bf16 [cos | sin] per id, id-major, into row b of out
+ * (row stride ldo elements, >= n_ids * dim): SDXL's add_time_proj(time_ids) written straight into columns 1280.. of add_embeds. */
+int dllm_time_ids_embedding(const float* ids, void* out, long ldo, int B, int n_ids, int dim, void* stream);
+/* y = silu(x) and dx = dy * silu'(x), bf16, n % 8 == 0. */
+int dllm_silu_bf16(const void* x, void* y, long n, void* stream);
+int dllm_silu_bwd_bf16(const void* dy, const void* x, void* dx, long n, void* stream);
+/* dst[b, r, :] = scale * src[b, :] for src [B, H], dst [B, R, H] bf16 (H % 8 == 0): backward of a mean over R rows. */
+int dllm_broadcast_rows(const void* src, void* dst, int B, int R, int H, float scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
