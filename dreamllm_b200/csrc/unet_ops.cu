@@ -172,11 +172,17 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_partial_kernel(const bf16* _
     partial[((static_cast<size_t>(n) * nchunks + chunk) * G + g) * 2 + which] = a;
   }
 }
-// forward: stats[n, g] = {mean, rstd};  backward (eps < 0): sums[n, g] = {sum g / count, sum g xhat / count}
+// forward: stats[n, g] = {mean, rstd};  backward (eps < 0, x unused): sums[n, g] = {sum g / count, sum g xhat / count}
 // One WARP per (n, g): lanes stride over the chunk partials, then a fixed-order shuffle tree (deterministic).  (One thread walking up
 // to 128 partials serially cost 17 us per GroupNorm on the VAE's 512x512 planes.)
-__global__ void gn_finalize_kernel(const float* __restrict__ partial, float* __restrict__ stats, int nchunks, int G, float count,
-                                   float eps, int total) {
+// The variance E[x^2] - mean^2 of the partials cancels in fp32 when |mean| >> std: at mean / std = 64 and 128 it put rstd off by 3e-4
+// to 9e-4 (H100, 700 W; tests/test_tower_kernels_gpu.py).  When mean^2 > kGnRecomputeRatio * var the warp re-reads the group and takes
+// the variance about the mean, sum (x - mean)^2 / count less the (sum (x - mean))^2 / count^2 correction: rstd then within 6e-5 at
+// mean / std = 128 on a 256 x 256 plane.  Below that ratio (|mean| < 11.3 std) the one-pass rstd is good to ~3e-5 and is kept bit for
+// bit, so ordinary activations pay nothing and compute what they computed before.
+constexpr float kGnRecomputeRatio = 128.f;
+__global__ void gn_finalize_kernel(const float* __restrict__ partial, const bf16* __restrict__ x, float* __restrict__ stats, int nchunks,
+                                   int G, int HW, int C, float count, float eps, int total) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // n * G + g
   const int lane = threadIdx.x & 31;
   if (i >= total) return;
@@ -189,14 +195,29 @@ __global__ void gn_finalize_kernel(const float* __restrict__ partial, float* __r
   }
   a = warp_sum(a);
   b = warp_sum(b);
-  if (lane != 0) return;
   if (eps < 0.f) {
+    if (lane != 0) return;
     stats[2 * i] = a / count;
     stats[2 * i + 1] = b / count;
     return;
   }
   const float mean = a / count;
-  const float var = fmaxf(b / count - mean * mean, 0.f);
+  float var = fmaxf(b / count - mean * mean, 0.f);
+  if (mean * mean > kGnRecomputeRatio * var) {   // the whole warp takes this branch (a, b are warp-uniform)
+    const int cpg = C / G;
+    const bf16* xg = x + static_cast<size_t>(n) * HW * C + static_cast<size_t>(g) * cpg;
+    float s1 = 0.f, s2 = 0.f;
+    for (int r = lane; r < HW; r += 32)
+      for (int c = 0; c < cpg; ++c) {
+        const float d = __bfloat162float(xg[static_cast<size_t>(r) * C + c]) - mean;
+        s1 += d;
+        s2 += d * d;
+      }
+    s1 = warp_sum(s1);
+    s2 = warp_sum(s2);
+    var = fmaxf((s2 - s1 * s1 / count) / count, 0.f);
+  }
+  if (lane != 0) return;
   stats[2 * i] = mean;
   stats[2 * i + 1] = rsqrtf(var + eps);
 }
@@ -309,7 +330,8 @@ static int gn_launch_stats(const bf16* x, float* stats, float* partial, int N, i
   const int nchunks = (HW + rows - 1) / rows;
   gn_partial_kernel<false><<<dim3(nchunks, N), m.threads, static_cast<size_t>(m.RL) * 2 * C * sizeof(float), s>>>(
       x, nullptr, nullptr, nullptr, nullptr, partial, HW, C, G, rows, m.RL, 0);
-  gn_finalize_kernel<<<(N * G * 32 + 255) / 256, 256, 0, s>>>(partial, stats, nchunks, G, static_cast<float>(HW) * (C / G), eps, N * G);
+  gn_finalize_kernel<<<(N * G * 32 + 255) / 256, 256, 0, s>>>(partial, x, stats, nchunks, G, HW, C, static_cast<float>(HW) * (C / G), eps,
+                                                               N * G);
   return 0;
 }
 static void gn_launch_apply(const bf16* x, const bf16* w, const bf16* b, const float* stats, bf16* y, int N, int HW, int C, int G, int silu,
@@ -430,18 +452,21 @@ __global__ void copy_cols_kernel(const bf16* __restrict__ src, bf16* __restrict_
   *reinterpret_cast<uint4*>(dst + r * Cd + col0 + v * 8) = reinterpret_cast<const uint4*>(src + r * Cs)[v];
 }
 int upsample2x_nhwc(const void* x, void* y, int N, int H, int W, int C, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(x, y);
   if (C % 8) return DLLM_ERR_SHAPE;
   const long total = static_cast<long>(N) * 4 * H * W * (C / 8);
   upsample2x_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>((const bf16*)x, (bf16*)y, N, H, W, C);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 int im2col_s2_nhwc(const void* x, void* out, int N, int H, int W, int C, int pad, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(x, out);
   if (C % 8 || H % 2 || W % 2) return DLLM_ERR_SHAPE;
   const long total = static_cast<long>(N) * (H / 2) * (W / 2) * 9 * (C / 8);
   im2col_s2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>((const bf16*)x, (bf16*)out, N, H, W, C, pad);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 int copy_cols(const void* src, void* dst, long rows, int Cs, int Cd, int col0, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(src, dst);
   if (Cs % 8 || Cd % 8 || col0 % 8 || rows <= 0) return DLLM_ERR_SHAPE;
   const long total = rows * (Cs / 8);
   copy_cols_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>((const bf16*)src, (bf16*)dst, rows, Cs, Cd, col0);
@@ -678,7 +703,8 @@ int groupnorm_bwd_nhwc(const void* dy, const void* x, const void* w, const void*
   float* sums = partial + static_cast<size_t>(N) * nchunks * G * 2;
   gn_partial_kernel<true><<<dim3(nchunks, N), m.threads, static_cast<size_t>(m.RL) * 2 * C * sizeof(float), s>>>(
       (const bf16*)x, (const bf16*)dy, (const bf16*)w, (const bf16*)b, stats, partial, HW, C, G, rows, m.RL, silu);
-  gn_finalize_kernel<<<(N * G * 32 + 255) / 256, 256, 0, s>>>(partial, sums, nchunks, G, static_cast<float>(HW) * (C / G), -1.f, N * G);
+  gn_finalize_kernel<<<(N * G * 32 + 255) / 256, 256, 0, s>>>(partial, nullptr, sums, nchunks, G, HW, C, static_cast<float>(HW) * (C / G),
+                                                               -1.f, N * G);
   int arows = 128;
   while (arows > m.RL && static_cast<long>(N) * ((HW + arows - 1) / arows) < 4 * num_sms()) arows /= 2;
   gn_apply_kernel<true><<<dim3((HW + arows - 1) / arows, N), m.threads, 0, s>>>((const bf16*)x, (const bf16*)dy, (const bf16*)w,
@@ -880,6 +906,7 @@ int col2im_s2_nhwc(const void* dcols, void* dx, int N, int H, int W, int C, cuda
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 int copy_cols2(const void* src, void* dst, long rows, int Cs, int Cd, int scol0, int dcol0, int ncols, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(src, dst);
   if (Cs % 8 || Cd % 8 || scol0 % 8 || dcol0 % 8 || ncols % 8 || rows <= 0) return DLLM_ERR_SHAPE;
   const long total = rows * (ncols / 8);
   copy_cols2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>((const bf16*)src, (bf16*)dst, rows, Cs, Cd, scol0, dcol0, ncols);

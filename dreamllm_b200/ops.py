@@ -515,7 +515,7 @@ def groupnorm(x_nhwc, weight, bias, groups, eps, silu, return_stats=False):
 
 
 def groupnorm_bwd(dy, x_nhwc, weight, bias, stats, groups, silu, dres=None):
-    _chk_cuda(dy, x_nhwc, stats, dres)
+    _chk_cuda(dy, x_nhwc, weight, bias, stats, dres)
     N, C = x_nhwc.shape[0], x_nhwc.shape[-1]
     HW = x_nhwc.numel() // (N * C)
     assert dy.is_contiguous() and x_nhwc.is_contiguous() and (dres is None or dres.is_contiguous())
@@ -539,8 +539,10 @@ def layernorm_bwd(dy2d, x2d, weight, eps, dres=None):
 
 
 def geglu_bwd(dout2d, in2d):
+    _chk_cuda(dout2d, in2d)
     T, I2 = in2d.shape
-    assert dout2d.is_contiguous() and in2d.is_contiguous()
+    assert dout2d.dtype == BF16 and in2d.dtype == BF16 and dout2d.is_contiguous() and in2d.is_contiguous()
+    assert dout2d.shape == (T, I2 // 2)
     din = torch.empty_like(in2d)
     check(lib().dllm_geglu_bwd(_p(dout2d), _p(in2d), _p(din), T, I2 // 2, _stream()), "dllm_geglu_bwd")
     LAUNCHES.add(1)
@@ -577,7 +579,10 @@ def attn_fwd_cross_lse(q, k, v, scale=None):
 
 
 def upsample2x_bwd(dy_nhwc):
+    _chk_cuda(dy_nhwc)
+    assert dy_nhwc.dtype == BF16 and dy_nhwc.is_contiguous()
     N, H2, W2, C = dy_nhwc.shape
+    assert H2 % 2 == 0 and W2 % 2 == 0
     dx = torch.empty((N, H2 // 2, W2 // 2, C), device=dy_nhwc.device, dtype=BF16)
     check(lib().dllm_upsample2x_bwd_nhwc(_p(dy_nhwc), _p(dx), N, H2 // 2, W2 // 2, C, _stream()), "dllm_upsample2x_bwd_nhwc")
     LAUNCHES.add(1)
@@ -585,6 +590,8 @@ def upsample2x_bwd(dy_nhwc):
 
 
 def col2im_s2(dcols2d, N, H, W, C):
+    _chk_cuda(dcols2d)
+    assert dcols2d.dtype == BF16 and dcols2d.is_contiguous() and dcols2d.shape == (N * (H // 2) * (W // 2), 9 * C)
     dx = torch.empty((N, H, W, C), device=dcols2d.device, dtype=BF16)
     check(lib().dllm_col2im_s2_nhwc(_p(dcols2d), _p(dx), N, H, W, C, _stream()), "dllm_col2im_s2_nhwc")
     LAUNCHES.add(1)
@@ -614,6 +621,9 @@ def split_channels(x_nhwc, c_first):
 
 
 def conv_out_bwd(deps_nchw_f32, weight, C):
+    _chk_cuda(deps_nchw_f32, weight)
+    assert deps_nchw_f32.dtype == torch.float32 and deps_nchw_f32.is_contiguous()
+    assert weight.dtype == BF16 and weight.is_contiguous() and weight.shape[:2] == (deps_nchw_f32.shape[1], C)
     B, Cout, H, W = deps_nchw_f32.shape
     dx = torch.empty((B, H, W, C), device=weight.device, dtype=BF16)
     check(lib().dllm_conv_out_bwd(_p(deps_nchw_f32), _p(weight), _p(dx), B, C, H, W, Cout, _stream()), "dllm_conv_out_bwd")
@@ -622,6 +632,8 @@ def conv_out_bwd(deps_nchw_f32, weight, C):
 
 
 def timestep_embedding_batch(t_i32, dim):
+    _chk_cuda(t_i32)
+    assert t_i32.dtype == torch.int32 and t_i32.is_contiguous()
     B = t_i32.numel()
     out = torch.empty((B, dim), device=t_i32.device, dtype=BF16)
     check(lib().dllm_timestep_embedding_batch(_p(t_i32), _p(out), B, dim, _stream()), "dllm_timestep_embedding_batch")
@@ -668,6 +680,8 @@ def geglu(x2d):
 
 
 def upsample2x(x_nhwc):
+    _chk_cuda(x_nhwc)
+    assert x_nhwc.dtype == BF16 and x_nhwc.is_contiguous()
     N, H, W, C = x_nhwc.shape
     y = torch.empty((N, 2 * H, 2 * W, C), device=x_nhwc.device, dtype=BF16)
     check(lib().dllm_upsample2x_nhwc(_p(x_nhwc), _p(y), N, H, W, C, _stream()), "dllm_upsample2x_nhwc")
@@ -676,6 +690,8 @@ def upsample2x(x_nhwc):
 
 
 def im2col_s2(x_nhwc, pad=1):
+    _chk_cuda(x_nhwc)
+    assert x_nhwc.dtype == BF16 and x_nhwc.is_contiguous() and pad in (0, 1)
     N, H, W, C = x_nhwc.shape
     out = torch.empty((N * (H // 2) * (W // 2), 9 * C), device=x_nhwc.device, dtype=BF16)
     check(lib().dllm_im2col_s2_nhwc(_p(x_nhwc), _p(out), N, H, W, C, int(pad), _stream()), "dllm_im2col_s2_nhwc")
@@ -765,6 +781,10 @@ def conv_out(x_nhwc, weight, bias, out=None):
 
 
 def timestep_embedding(timesteps_i32, step_i32, B, dim):
+    """emb [B, dim] of t = timesteps_i32[step_i32[0]], both read on the device (one captured graph serves every step)."""
+    _chk_cuda(timesteps_i32, step_i32)
+    assert timesteps_i32.dtype == torch.int32 and timesteps_i32.is_contiguous()
+    assert step_i32.dtype == torch.int32 and step_i32.numel() >= 1
     out = torch.empty((B, dim), device=timesteps_i32.device, dtype=BF16)
     check(lib().dllm_timestep_embedding(_p(timesteps_i32), _p(step_i32), _p(out), B, dim, _stream()), "dllm_timestep_embedding")
     LAUNCHES.add(1)
@@ -788,8 +808,12 @@ def softmax_rows_(x2d, scale):
 
 
 def vae_sample(h_nchw_f32, wq, bq, z_f32, scaling):
+    _chk_cuda(h_nchw_f32, wq, bq, z_f32)
     B, C2, H, W = h_nchw_f32.shape
     L = C2 // 2
+    assert h_nchw_f32.dtype == torch.float32 and h_nchw_f32.is_contiguous()
+    assert z_f32.dtype == torch.float32 and z_f32.is_contiguous() and z_f32.shape == (B, L, H, W)
+    assert wq.dtype == BF16 and wq.is_contiguous() and wq.numel() == C2 * C2 and bq.dtype == BF16 and bq.numel() == C2
     out = torch.empty((B, L, H, W), device=h_nchw_f32.device, dtype=torch.float32)
     check(lib().dllm_vae_sample(_p(h_nchw_f32), _p(wq), _p(bq), _p(z_f32), _p(out), B, L, H * W, float(scaling), _stream()), "dllm_vae_sample")
     LAUNCHES.add(1)
