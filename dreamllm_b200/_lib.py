@@ -11,7 +11,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.environ.get("DLLM_LIB_PATH") or os.path.join(_HERE, "libdreamllm_sm100.so")   # env override: A/B builds in dev scripts
-SOURCES = ["capi.cu", "gemm_sm90.cu", "elementwise.cu", "attn_sm90.cu", "unet_ops.cu", "optim.cu", "sdxl_ops.cu"]
+SOURCES = ["capi.cu", "gemm_sm90.cu", "elementwise.cu", "attn_sm90.cu", "unet_ops.cu", "optim.cu", "sdxl_ops.cu", "decode_sm90.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
@@ -139,6 +139,10 @@ SIGNATURES = {
     "dllm_silu_bf16": (_i, [_vp, _vp, _l, _vp]),
     "dllm_silu_bwd_bf16": (_i, [_vp, _vp, _vp, _l, _vp]),
     "dllm_broadcast_rows": (_i, [_vp, _vp, _i, _i, _i, _f, _vp]),
+    "dllm_attn_decode_plan": (_i, [_i, _i, _i, _i, _vp, _vp]),
+    "dllm_attn_decode_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i]),
+    "dllm_attn_decode": (_i, [_vp, _l, _vp, _vp, _vp, _vp, _i, _vp, _l, _vp, _sz, _i, _i, _i, _i, _i, _f, _i, _vp]),
+    "dllm_rope_append_kv": (_i, [_vp, _l, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
 }
 
 _lib = None

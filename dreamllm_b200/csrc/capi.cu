@@ -376,5 +376,23 @@ int dllm_broadcast_rows(const void* src, void* dst, int B, int R, int H, float s
   ensure_context(src);
   return broadcast_rows(src, dst, B, R, H, scale, S(stream));
 }
+int dllm_attn_decode_plan(int B, int nkv, int max_len, int sms, int* n_splits, int* split_len) {
+  return attn_decode_plan(B, nkv, max_len, sms, n_splits, split_len);
+}
+size_t dllm_attn_decode_workspace_bytes(int B, int nh, int nkv, int d, int max_len, int sms) {
+  return attn_decode_workspace(B, nh, nkv, d, max_len, sms);
+}
+int dllm_attn_decode(const void* q, long ld_q, const void* k_cache, const void* v_cache, const int* kv_len, const void* kv_mask,
+                     int mask_ld, void* out, long ld_o, void* workspace, size_t workspace_bytes, int B, int max_len, int nh, int nkv, int d,
+                     float scale, int sms, void* stream) {
+  ensure_context(q);
+  return attn_decode(q, ld_q, k_cache, v_cache, kv_len, kv_mask, mask_ld, out, ld_o, workspace, workspace_bytes, B, max_len, nh, nkv, d,
+                     scale, sms, S(stream));
+}
+int dllm_rope_append_kv(void* qkv, long ld, const void* cos_table, const void* sin_table, const int* pos, void* k_cache, void* v_cache,
+                        const int* kv_len, int max_len, int B, int nh, int nkv, int d, void* stream) {
+  ensure_context(qkv);
+  return rope_append_kv(qkv, ld, cos_table, sin_table, pos, k_cache, v_cache, kv_len, max_len, B, nh, nkv, d, S(stream));
+}
 
 }  // extern "C"

@@ -105,4 +105,12 @@ int time_ids_embedding(const float* ids, void* out, long ldo, int B, int n_ids, 
 int silu_bf16(const void* x, void* y, long n, cudaStream_t s);
 int silu_bwd_bf16(const void* dy, const void* x, void* dx, long n, cudaStream_t s);
 int broadcast_rows(const void* src, void* dst, int B, int R, int H, float scale, cudaStream_t s);
+// decode_sm90.cu: one-token decode attention over the kv-cache (split-KV, cache length on the device) and the RoPE + cache append
+int attn_decode_plan(int B, int nkv, int max_len, int sms, int* n_splits, int* split_len);
+size_t attn_decode_workspace(int B, int nh, int nkv, int d, int max_len, int sms);
+int attn_decode(const void* q, long ld_q, const void* k_cache, const void* v_cache, const int* kv_len, const void* kv_mask, int mask_ld,
+                void* out, long ld_o, void* workspace, size_t ws_bytes, int B, int max_len, int nh, int nkv, int d, float scale, int sms,
+                cudaStream_t s);
+int rope_append_kv(void* qkv, long ld, const void* cos_t, const void* sin_t, const int* pos, void* k_cache, void* v_cache,
+                   const int* kv_len, int max_len, int B, int nh, int nkv, int d, cudaStream_t s);
 }  // namespace dllm

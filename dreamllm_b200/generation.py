@@ -69,6 +69,14 @@ def ragged(decode_one, input_ids, attention_mask, pad_id: int):
     return out
 
 
+def check_graph_decode(model):
+    """Refuse, before the prefill, what the captured decode step does not compute."""
+    cfg = model.config
+    if getattr(cfg, "output_attentions", False) or getattr(cfg, "log_attentions", False):
+        raise ValueError("output_attentions / log_attentions are not available with use_cuda_graph=True: the captured decode step does "
+                         "not compute attention probabilities")
+
+
 def _left_padded(attention_mask) -> bool:
     """True when every row's LAST prompt position is a real token (left padding, or no padding): the batched kv-cache path applies."""
     return bool(attention_mask[:, -1].all())
@@ -83,8 +91,10 @@ def _positions(attention_mask):
 @torch.no_grad()
 def generate(model, input_ids, images=None, max_new_tokens: int = 16, do_sample: bool = False, temperature: float = 1.0, top_k: int = 0,
              top_p: float = 1.0, repetition_penalty: float = 1.0, eos_token_id=None, pad_token_id=None, generator=None,
-             attention_mask=None, stopping_criteria=None):
-    """Prefill once with the kv-cache, then one cached decode step per token.  Finished rows keep emitting `pad_token_id` (HF semantics);
+             attention_mask=None, stopping_criteria=None, use_cuda_graph: bool = False):
+    """Prefill once with the kv-cache, then one cached decode step per token.  `use_cuda_graph=True` runs every decode step as one
+    replay of a captured graph (`decode.DecodeGraph`); the prefill and the token selection are unchanged, the logits differ from the
+    eager steps' only in the summation order of the attention.  Finished rows keep emitting `pad_token_id` (HF semantics);
     stops when every row has produced an EOS or a `stopping_criteria` callable `(input_ids, scores) -> bool | BoolTensor[B]` fires for it
     (HF `StoppingCriteria` semantics; the reference's VQA eval passes a keyword criterion, omni/eval/vqa/vqa_inference.py:105-106).
     Returns [B, S + n_generated] ids (prompt included, like HF for decoder-only models)."""
@@ -97,7 +107,7 @@ def generate(model, input_ids, images=None, max_new_tokens: int = 16, do_sample:
             raise NotImplementedError("right-padded prompt batches with images: left-pad them (HF's convention for decoder-only models) or "
                                       "pass the prompts one at a time (images are matched to <im_start> tokens in batch order)")
         return ragged(lambda ids: generate(model, ids, None, max_new_tokens, do_sample, temperature, top_k, top_p, repetition_penalty,
-                                           eos_token_id, pad_token_id, generator, None, stopping_criteria),
+                                           eos_token_id, pad_token_id, generator, None, stopping_criteria, use_cuda_graph),
                       input_ids, attention_mask, pad_token_id if pad_token_id is not None else
                       (eos_token_id if isinstance(eos_token_id, int) else (eos_token_id[0] if eos_token_id else 0)))
     eos = None
@@ -113,25 +123,37 @@ def generate(model, input_ids, images=None, max_new_tokens: int = 16, do_sample:
     # left-padded batch: ONE batched prefill + batched decode steps; the pad keys stay masked inside the kv-cache and RoPE positions come
     # from the mask, exactly as HF generate drives the reference (vqa_inference.py:112-130, modeling_dreamllm.py:1511-1547)
     mask_kw = {} if am is None else dict(attention_mask=am, position_ids=_positions(am))
+    if use_cuda_graph:
+        check_graph_decode(model)
     out = model(input_ids=input_ids, images=images, use_cache=True, last_token_logits_only=True, **mask_kw)
     cache = out.past_key_values
+    logits = out.logits[:, -1]
+    graph = None
+    if use_cuda_graph:
+        from .decode import DecodeGraph
+        graph = DecodeGraph(model, cache, input_ids.shape[0], positions=None if am is None else am.long().sum(-1))
     for i in range(max_new_tokens):
-        nxt = pick_next_token(out.logits[:, -1], seq, do_sample=do_sample, generator=generator, **warp)
+        nxt = pick_next_token(logits, seq, do_sample=do_sample, generator=generator, **warp)
         if pad_token_id is not None:
             nxt = torch.where(unfinished, nxt, torch.full_like(nxt, pad_token_id))       # finished rows keep emitting pad
         if eos is not None:
             unfinished = unfinished & ~torch.isin(nxt, eos)
         seq = torch.cat([seq, nxt[:, None]], 1)
         for crit in (stopping_criteria or ()):
-            done = crit(seq, out.logits[:, -1])
+            done = crit(seq, logits)
             done = torch.as_tensor(done, device=seq.device, dtype=torch.bool)
             unfinished = unfinished & ~(done.expand_as(unfinished))
         if i + 1 == max_new_tokens or ((eos is not None or stopping_criteria) and not bool(unfinished.any())):
             break
+        if graph is not None:
+            graph.ids.copy_(nxt)
+            logits = graph.replay()
+            continue
         if am is not None:
             am = torch.cat([am, torch.ones_like(am[:, :1])], 1)
             mask_kw = dict(attention_mask=am, position_ids=am.long().sum(-1, keepdim=True) - 1)
         out = model(input_ids=nxt[:, None], past_key_values=cache, use_cache=True, last_token_logits_only=True, **mask_kw)
+        logits = out.logits[:, -1]
     return seq
 
 
@@ -145,7 +167,7 @@ def _gather_beams(t: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def beam_search(model, input_ids, images=None, num_beams: int = 5, max_new_tokens: int = 16, length_penalty: float = 1.0,
                 early_stopping=False, eos_token_id=None, pad_token_id=None, stopping_criteria=None,
-                length_normalization: str = "generated", return_scores: bool = False, attention_mask=None):
+                length_normalization: str = "generated", return_scores: bool = False, attention_mask=None, use_cuda_graph: bool = False):
     """Beam search over the kv-cache decode path — what `model.generate(..., num_beams=5)` does in the reference's default VQA eval
     (omni/eval/vqa/vqa_inference.py:111-119, `--beamsearch True` is the default, omni/utils/eval_utils.py:141).
 
@@ -156,6 +178,7 @@ def beam_search(model, input_ids, images=None, num_beams: int = 5, max_new_token
     `GenerationMixin.generate(num_beams=...)` on random LLaMAs; `"total"` divides by prompt + generated length, the rule of the 4.35.x
     scorer the reference pins (restated from memory: that version cannot be installed here, so this mode is unpinned).
     The prompt is prefilled once per sample; the cache is then repeated per beam and re-ordered in place every step.
+    `use_cuda_graph=True` runs the decode steps as replays of one captured graph (`decode.DecodeGraph`), as in `generate`.
     Returns [B, prompt + generated] ids of the best hypothesis per sample (padded with `pad_token_id` after EOS)."""
     if length_normalization not in ("generated", "total"):
         raise ValueError("length_normalization must be 'generated' or 'total'")
@@ -191,11 +214,17 @@ def beam_search(model, input_ids, images=None, num_beams: int = 5, max_new_token
         if not _left_padded(am):
             raise ValueError("beam search over a padded batch needs LEFT padding (HF's convention for decoder-only models)")
     mask_kw = {} if am is None else dict(attention_mask=am, position_ids=_positions(am))
+    if use_cuda_graph:
+        check_graph_decode(model)
     out = model(input_ids=input_ids, images=images, use_cache=True, last_token_logits_only=True, **mask_kw)
     cache = out.past_key_values
     cache.repeat_interleave(k)
     if am is not None:
         am = am.repeat_interleave(k, dim=0)
+    graph = None
+    if use_cuda_graph:                                                   # built after repeat_interleave, which reallocates the cache
+        from .decode import DecodeGraph
+        graph = DecodeGraph(model, cache, B * k, positions=None if am is None else am.long().sum(-1))
     logits = out.logits[:, -1].float().repeat_interleave(k, dim=0)      # [B*k, V]
     cur_len = prompt_len
     while True:
@@ -244,6 +273,10 @@ def beam_search(model, input_ids, images=None, num_beams: int = 5, max_new_token
         if not more:
             break
         cache.reorder((next_src + torch.arange(B, device=dev)[:, None] * k).reshape(-1))
+        if graph is not None:
+            graph.ids.copy_(running[:, :, cur_len - 1].reshape(B * k))
+            logits = graph.replay()
+            continue
         if am is not None:                                               # (rows of one sample share a mask: re-ordering beams keeps it)
             am = torch.cat([am, torch.ones_like(am[:, :1])], 1)
             mask_kw = dict(attention_mask=am, position_ids=am.long().sum(-1, keepdim=True) - 1)

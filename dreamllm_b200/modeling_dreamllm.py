@@ -415,7 +415,8 @@ class KVCache:
         self.mask[:, :L] = attention_mask.to(device=self.mask.device, dtype=torch.uint8)
 
     def repeat_interleave(self, k: int):
-        """Beam search: every sample's cache rows repeated k times along the batch dimension (in place)."""
+        """Beam search: every sample's cache rows repeated k times along the batch dimension.  The buffers are reallocated: build a
+        `decode.DecodeGraph` after this call, not before."""
         for li in range(len(self.k)):
             self.k[li] = self.k[li].repeat_interleave(k, dim=0)
             self.v[li] = self.v[li].repeat_interleave(k, dim=0)
@@ -425,14 +426,14 @@ class KVCache:
 
     def reorder(self, beam_idx):
         """Beam search: row b takes the history of row beam_idx[b] (reference `_reorder_cache`, :1549-1554).  Only the valid prefix
-        [:len] is moved."""
+        [:len] is moved.  In place: every buffer keeps its address, so a captured `decode.DecodeGraph` stays valid across a reorder."""
         L = self.len
         for li in range(len(self.k)):
             idx = beam_idx.to(self.k[li].device)
             self.k[li][:, :L] = self.k[li][:, :L].index_select(0, idx)
             self.v[li][:, :L] = self.v[li][:, :L].index_select(0, idx)
         if self.mask is not None:
-            self.mask = self.mask.index_select(0, beam_idx.to(self.mask.device)).contiguous()
+            self.mask.copy_(self.mask.index_select(0, beam_idx.to(self.mask.device)))
         return self
 
 
@@ -1228,9 +1229,10 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
     @torch.no_grad()
     def generate(self, input_ids, images=None, max_new_tokens=16, do_sample=False, temperature=1.0, top_k=0, top_p=1.0,
                  repetition_penalty=1.0, eos_token_id=None, pad_token_id=None, generator=None, attention_mask=None,
-                 stopping_criteria=None, **kwargs):
+                 stopping_criteria=None, use_cuda_graph=False, **kwargs):
         """Decoding with the kv-cache (what HF `generate` does through the reference: omni/eval/vqa/vqa_inference.py:112-130): greedy or
-        temperature / top-k / top-p sampling with HF's processor semantics, or beam search with `num_beams > 1` (dreamllm_b200/generation.py)."""
+        temperature / top-k / top-p sampling with HF's processor semantics, or beam search with `num_beams > 1` (dreamllm_b200/generation.py).
+        `use_cuda_graph=True` replays each decode step from one captured CUDA graph (dreamllm_b200/decode.py)."""
         from .generation import beam_search, generate
         num_beams = int(kwargs.get("num_beams", 1))
         if num_beams > 1:                                      # the reference's default VQA eval: num_beams=5 (vqa_inference.py:111-119)
@@ -1242,16 +1244,18 @@ class DreamLLMForCausalMLM(DreamLLMPreTrainedModel):
                 from .generation import ragged
                 kw = dict(kwargs)
                 return ragged(lambda ids: self.generate(ids, max_new_tokens=max_new_tokens, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
-                                                        stopping_criteria=stopping_criteria, **kw), input_ids, attention_mask,
+                                                        stopping_criteria=stopping_criteria, use_cuda_graph=use_cuda_graph, **kw),
+                              input_ids, attention_mask,
                               pad_token_id if pad_token_id is not None else (eos_token_id if isinstance(eos_token_id, int) else 0))
             return beam_search(self, input_ids, images=images, num_beams=num_beams, max_new_tokens=max_new_tokens,
                                length_penalty=kwargs.get("length_penalty", 1.0), early_stopping=kwargs.get("early_stopping", False),
                                eos_token_id=eos_token_id, pad_token_id=pad_token_id, stopping_criteria=stopping_criteria,
-                               length_normalization=kwargs.get("length_normalization", "generated"), attention_mask=attention_mask)
+                               length_normalization=kwargs.get("length_normalization", "generated"), attention_mask=attention_mask,
+                               use_cuda_graph=use_cuda_graph)
         return generate(self, input_ids, images=images, max_new_tokens=max_new_tokens, do_sample=do_sample, temperature=temperature,
                         top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, eos_token_id=eos_token_id,
                         pad_token_id=pad_token_id, generator=generator, attention_mask=attention_mask,
-                        stopping_criteria=stopping_criteria)
+                        stopping_criteria=stopping_criteria, use_cuda_graph=use_cuda_graph)
 
     @torch.no_grad()
     def generate_greedy(self, input_ids, max_new_tokens=16, images=None, eos_token_id=None):

@@ -6,6 +6,7 @@ fallback: a CPU tensor is an error.
 """
 from __future__ import annotations
 
+import ctypes
 import weakref
 
 import torch
@@ -868,6 +869,66 @@ def attn_probs(q, k, lse, causal=True, seqlens=None, kv_len=None, kv_mask=None, 
                                     q.stride(1), k.stride(1), int(causal), scale, _stream()), "dllm_attn_probs_gqa")
     LAUNCHES.add(1)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ one-token decode (decode.py)
+def attn_decode_plan(B, nkv, max_len, sms=0):
+    """(n_splits, split_len) of `attn_decode` for these sizes; sms <= 0 = the current device's SM count."""
+    ns, sl = ctypes.c_int(0), ctypes.c_int(0)
+    check(lib().dllm_attn_decode_plan(int(B), int(nkv), int(max_len), int(sms), ctypes.byref(ns), ctypes.byref(sl)), "dllm_attn_decode_plan")
+    return ns.value, sl.value
+
+
+def attn_decode_workspace_bytes(B, nh, nkv, d, max_len, sms=0):
+    return int(lib().dllm_attn_decode_workspace_bytes(int(B), int(nh), int(nkv), int(d), int(max_len), int(sms)))
+
+
+def attn_decode(q, k_cache, v_cache, kv_len, kv_mask=None, workspace=None, out=None, scale=None, sms=0):
+    """Attention of ONE new token per row over the first `kv_len` rows of the cache (all visible to it).
+    q [B, nh, d] view (heads contiguous, e.g. the q columns of the fused qkv row); k_cache / v_cache [B, max_len, nkv, d] contiguous;
+    kv_len: int32 device tensor (its first element is read by the kernel, so a captured launch follows the cache as it grows);
+    kv_mask: uint8 [B, mask_ld] (0 = padded key), as `attn_fwd_cache`.  workspace: uint8 of at least `attn_decode_workspace_bytes`
+    (allocated here when None).  Returns out [B, nh * d] bf16.  Deterministic: the split partials are merged in a fixed order."""
+    _chk_cuda(q, k_cache, v_cache, kv_len, kv_mask, workspace, out)
+    B, nh, d = q.shape
+    max_len, nkv = k_cache.shape[1], k_cache.shape[2]
+    assert q.dtype == BF16 and q.stride(2) == 1 and q.stride(1) == d
+    for t in (k_cache, v_cache):
+        assert t.dtype == BF16 and t.is_contiguous() and tuple(t.shape) == (B, max_len, nkv, d)
+    assert kv_len.dtype == torch.int32 and kv_len.numel() >= 1
+    mask_ld = 0
+    if kv_mask is not None:
+        assert kv_mask.dtype == torch.uint8 and kv_mask.dim() == 2 and kv_mask.shape[0] == B and kv_mask.stride(1) == 1
+        mask_ld = kv_mask.stride(0)
+    wsb = attn_decode_workspace_bytes(B, nh, nkv, d, max_len, sms)
+    if workspace is None:
+        workspace = torch.empty(wsb, device=q.device, dtype=torch.uint8)
+    assert workspace.dtype == torch.uint8 and workspace.numel() >= wsb
+    if out is None:
+        out = torch.empty((B, nh * d), device=q.device, dtype=BF16)
+    assert out.dtype == BF16 and out.shape == (B, nh * d) and out.stride(1) == 1
+    scale = float(d) ** -0.5 if scale is None else float(scale)
+    check(lib().dllm_attn_decode(_p(q), q.stride(0), _p(k_cache), _p(v_cache), _p(kv_len), _p(kv_mask), mask_ld, _p(out), out.stride(0),
+                                 _p(workspace), workspace.numel(), B, max_len, nh, nkv, d, scale, int(sms), _stream()), "dllm_attn_decode")
+    LAUNCHES.add(2)
+    return out
+
+
+def rope_append_kv_(qkv, cos_t, sin_t, pos_i32, k_cache, v_cache, kv_len, num_heads, num_kv_heads, head_dim):
+    """qkv [B, (nh + 2 nkv) d] (one new token per row): q and k rotated in place at positions pos_i32 [B] (`rope_`'s arithmetic), then
+    the rotated k and the v written to row kv_len[0] (int32 device tensor) of k_cache / v_cache [B, max_len, nkv, d]."""
+    _chk_cuda(qkv, cos_t, sin_t, pos_i32, k_cache, v_cache, kv_len)
+    B = qkv.shape[0]
+    max_len = k_cache.shape[1]
+    assert qkv.dtype == BF16 and qkv.stride(1) == 1 and qkv.shape[1] >= (num_heads + 2 * num_kv_heads) * head_dim
+    assert pos_i32.dtype == torch.int32 and pos_i32.is_contiguous() and pos_i32.numel() == B and kv_len.dtype == torch.int32
+    assert cos_t.dtype == BF16 and cos_t.is_contiguous() and cos_t.shape[1] == head_dim
+    for t in (k_cache, v_cache):
+        assert t.dtype == BF16 and t.is_contiguous() and tuple(t.shape) == (B, max_len, num_kv_heads, head_dim)
+    check(lib().dllm_rope_append_kv(_p(qkv), qkv.stride(0), _p(cos_t), _p(sin_t), _p(pos_i32), _p(k_cache), _p(v_cache), _p(kv_len),
+                                    max_len, B, num_heads, num_kv_heads, head_dim, _stream()), "dllm_rope_append_kv")
+    LAUNCHES.add(1)
+    return qkv
 
 
 # ------------------------------------------------------------------------------------------------ SDXL addition embedding

@@ -271,6 +271,28 @@ int dllm_silu_bwd_bf16(const void* dy, const void* x, void* dx, long n, void* st
 /* dst[b, r, :] = scale * src[b, :] for src [B, H], dst [B, R, H] bf16 (H % 8 == 0): backward of a mean over R rows. */
 int dllm_broadcast_rows(const void* src, void* dst, int B, int R, int H, float scale, void* stream);
 
+/* ---- One-token decode step over the kv-cache (dreamllm_b200/decode.py captures it in a CUDA graph).  The cache length is read from
+ * the device (`kv_len`, one int32 for the whole batch), so a captured launch stays valid as the cache grows. ----
+ * Split planner: the kv rows [0, max_len) are cut into n_splits ranges of split_len rows (a multiple of 64).  split_len depends on
+ * (B, nkv, sms) only; max_len only sets n_splits, and the last split starts below max_len.  sms <= 0: the current device's SM count. */
+int dllm_attn_decode_plan(int B, int nkv, int max_len, int sms, int* n_splits, int* split_len);
+/* fp32 partials of one dllm_attn_decode call with these sizes (the same sms): n_splits * B * nh * (d + 2) * 4 bytes. */
+size_t dllm_attn_decode_workspace_bytes(int B, int nh, int nkv, int d, int max_len, int sms);
+/* out[b, h * d : (h + 1) * d] = softmax(q[b, h] . K[b, :kv_len, h / g]^T * scale + mask) . V[b, :kv_len, h / g]  (g = nh / nkv in
+ * {1, 2, 4, 8}, d 64 or 128).  q: row b at q + b * ld_q (16-byte aligned, ld_q % 8 == 0), heads of d contiguous (the q columns of
+ * the fused qkv row).  k_cache / v_cache:
+ * contiguous [B, max_len, nkv, d].  kv_mask (nullable): uint8 [B, mask_ld >= max_len], 0 = padded key.  Every key below *kv_len is
+ * visible (the query is the newest token).  out row stride ld_o.  Splits at or past *kv_len write a neutral partial; a combine kernel
+ * merges the partials in fixed order (deterministic, no atomics). */
+int dllm_attn_decode(const void* q, long ld_q, const void* k_cache, const void* v_cache, const int* kv_len, const void* kv_mask,
+                     int mask_ld, void* out, long ld_o, void* workspace, size_t workspace_bytes, int B, int max_len, int nh, int nkv, int d,
+                     float scale, int sms, void* stream);
+/* qkv [B, (nh + 2 nkv) d] (row stride ld): q and k heads rotated in place at positions pos[B] (int32) with the bf16 cos / sin tables
+ * of dllm_rope_inplace (same arithmetic, same bits); the rotated k and the v of row b are written to row *kv_len of k_cache / v_cache
+ * [B, max_len, nkv, d].  Nothing is written to the cache when *kv_len >= max_len. */
+int dllm_rope_append_kv(void* qkv, long ld, const void* cos_table, const void* sin_table, const int* pos, void* k_cache, void* v_cache,
+                        const int* kv_len, int max_len, int B, int nh, int nkv, int d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
