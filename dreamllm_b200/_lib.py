@@ -120,6 +120,10 @@ SIGNATURES = {
     "dllm_groupnorm_apply": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "dllm_groupnorm_bwd_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _i, _vp]),
     "dllm_layernorm_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
+    "dllm_layernorm_bwd_affine_workspace_bytes": (_sz, [_i, _i]),
+    "dllm_layernorm_bwd_affine": (_i, [_vp] * 8 + [_sz, _i, _i, _f, _vp]),
+    "dllm_quick_gelu": (_i, [_vp, _vp, _l, _vp]),
+    "dllm_quick_gelu_bwd": (_i, [_vp, _vp, _vp, _l, _vp]),
     "dllm_geglu_bwd": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
     "dllm_upsample2x_bwd_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "dllm_col2im_s2_nhwc": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),

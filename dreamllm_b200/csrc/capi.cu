@@ -294,6 +294,20 @@ int dllm_layernorm_bwd(const void* dy, const void* x, const void* w, const void*
   ensure_context(dy);
   return layernorm_bwd(dy, x, w, dres, dx, T, H, eps, S(stream));
 }
+size_t dllm_layernorm_bwd_affine_workspace_bytes(int T, int H) { return layernorm_bwd_affine_workspace(T, H); }
+int dllm_layernorm_bwd_affine(const void* dy, const void* x, const void* w, const void* dres, void* dx, void* dgamma, void* dbeta,
+                              void* workspace, size_t workspace_bytes, int T, int H, float eps, void* stream) {
+  ensure_context(dy);
+  return layernorm_bwd_affine(dy, x, w, dres, dx, dgamma, dbeta, workspace, workspace_bytes, T, H, eps, S(stream));
+}
+int dllm_quick_gelu(const void* x, void* y, long n, void* stream) {
+  ensure_context(x);
+  return quick_gelu(x, y, n, S(stream));
+}
+int dllm_quick_gelu_bwd(const void* dy, const void* x, void* dx, long n, void* stream) {
+  ensure_context(dy);
+  return quick_gelu_bwd(dy, x, dx, n, S(stream));
+}
 int dllm_geglu_bwd(const void* dout, const void* in, void* din, int T, int I, void* stream) {
   ensure_context(dout);
   return geglu_bwd(dout, in, din, T, I, S(stream));

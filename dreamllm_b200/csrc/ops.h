@@ -80,6 +80,11 @@ int groupnorm_stats(const void* x, float* stats, void* workspace, size_t ws_byte
 int groupnorm_apply(const void* x, const void* w, const void* b, const float* stats, void* y, int N, int HW, int C, int G, int silu,
                     cudaStream_t s);
 int layernorm_bwd(const void* dy, const void* x, const void* w, const void* dres, void* dx, int T, int H, float eps, cudaStream_t s);
+size_t layernorm_bwd_affine_workspace(int T, int H);
+int layernorm_bwd_affine(const void* dy, const void* x, const void* w, const void* dres, void* dx, void* dgamma, void* dbeta,
+                         void* workspace, size_t ws_bytes, int T, int H, float eps, cudaStream_t s);
+int quick_gelu(const void* x, void* y, long n, cudaStream_t s);
+int quick_gelu_bwd(const void* dy, const void* x, void* dx, long n, cudaStream_t s);
 int geglu_bwd(const void* dout, const void* in, void* din, int T, int I, cudaStream_t s);
 int upsample2x_bwd_nhwc(const void* dy, void* dx, int N, int H, int W, int C, cudaStream_t s);
 int col2im_s2_nhwc(const void* dcols, void* dx, int N, int H, int W, int C, cudaStream_t s);

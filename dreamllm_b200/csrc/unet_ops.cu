@@ -728,10 +728,13 @@ int groupnorm_apply(const void* x, const void* w, const void* b, const float* st
 }
 
 // ---- LayerNorm backward (dx only), warp per row, statistics recomputed:  dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres)
-template <int VPL>
+// kStats (the affine backward below): lane 0 also stores the row's (mean, rstd) for the weight-gradient pass; dx is computed by the same
+// code either way, so the two entries give the same dx bits.
+template <int VPL, bool kStats = false>
 __global__ void __launch_bounds__(256) layernorm_bwd_warp_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
                                                                  const bf16* __restrict__ w, const bf16* __restrict__ dres,
-                                                                 bf16* __restrict__ dx, int T, int H, float eps) {
+                                                                 bf16* __restrict__ dx, int T, int H, float eps,
+                                                                 float2* __restrict__ stats = nullptr) {
   const int lane = threadIdx.x & 31;
   const long row = (static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   if (row >= T) return;
@@ -757,6 +760,9 @@ __global__ void __launch_bounds__(256) layernorm_bwd_warp_kernel(const bf16* __r
       for (int j = 0; j < 8; ++j) { const float d = xv[i][j] - mean; sq += d * d; }
   }
   const float rstd = rsqrtf(warp_sum(sq) / static_cast<float>(H) + eps);
+  if constexpr (kStats) {
+    if (lane == 0) stats[row] = make_float2(mean, rstd);
+  }
   float s1 = 0.f, s2 = 0.f;
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
@@ -801,6 +807,139 @@ int layernorm_bwd(const void* dy, const void* x, const void* w, const void* dres
   if (nvec <= 64) layernorm_bwd_warp_kernel<2><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps);
   else if (nvec <= 128) layernorm_bwd_warp_kernel<4><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps);
   else layernorm_bwd_warp_kernel<6><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+
+// ---- LayerNorm backward with the affine gradients (CLIP tower training).  dx: the warp kernel above with kStats, so it is bit-identical
+// to layernorm_bwd.  dgamma[h] = sum_t dy[t, h] * xhat[t, h], dbeta[h] = sum_t dy[t, h] (xhat = (x - mean) * rstd in fp32, as the dx
+// kernel forms it): the rmsnorm_bwd_dw pattern — CTA (32 column vectors, row split) keeps 8 row groups of fp32 sums, adds them through
+// shared memory in group order and writes one partial row per split; a second kernel adds the kLnSplits partials in split order.  No
+// atomics: the bits depend only on the inputs and (T, H).
+constexpr int kLnSplits = 64;
+__global__ void __launch_bounds__(256) layernorm_bwd_dwb_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
+                                                                const float2* __restrict__ stats, float* __restrict__ partial, int T,
+                                                                int H) {
+  __shared__ float sg[8][32][9], sb[8][32][9];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int v = blockIdx.x * 32 + tx;
+  const int nvec = H >> 3;
+  const int rows_per = (T + kLnSplits - 1) / kLnSplits;
+  const int r0 = blockIdx.y * rows_per;
+  const int r1 = min(T, r0 + rows_per);
+  float ag[8], ab[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) ag[j] = ab[j] = 0.f;
+  if (v < nvec) {
+#pragma unroll 2
+    for (int r = r0 + ty; r < r1; r += 8) {
+      const long off = static_cast<long>(r) * H;
+      float d[8], xx[8];
+      up8(reinterpret_cast<const V8*>(dy + off)[v], d);
+      up8(reinterpret_cast<const V8*>(x + off)[v], xx);
+      const float2 st = stats[r];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        ag[j] += d[j] * ((xx[j] - st.x) * st.y);
+        ab[j] += d[j];
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    sg[ty][tx][j] = ag[j];
+    sb[ty][tx][j] = ab[j];
+  }
+  __syncthreads();
+  if (ty == 0 && v < nvec) {
+    float* pg = partial + static_cast<size_t>(blockIdx.y) * 2 * H;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float g = 0.f, b = 0.f;
+#pragma unroll
+      for (int y = 0; y < 8; ++y) {
+        g += sg[y][tx][j];
+        b += sb[y][tx][j];
+      }
+      pg[v * 8 + j] = g;
+      pg[H + v * 8 + j] = b;
+    }
+  }
+}
+__global__ void __launch_bounds__(256) layernorm_dwb_final_kernel(const float* __restrict__ partial, bf16* __restrict__ dgamma,
+                                                                  bf16* __restrict__ dbeta, int H) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  float g = 0.f, b = 0.f;
+  for (int p = 0; p < kLnSplits; ++p) {
+    g += partial[static_cast<size_t>(p) * 2 * H + h];
+    b += partial[static_cast<size_t>(p) * 2 * H + H + h];
+  }
+  dgamma[h] = __float2bfloat16_rn(g);
+  dbeta[h] = __float2bfloat16_rn(b);
+}
+
+size_t layernorm_bwd_affine_workspace(int T, int H) {
+  if (T <= 0 || H <= 0) return 0;
+  return static_cast<size_t>(T) * sizeof(float2) + static_cast<size_t>(kLnSplits) * 2 * H * sizeof(float);
+}
+
+int layernorm_bwd_affine(const void* dy, const void* x, const void* w, const void* dres, void* dx, void* dgamma, void* dbeta,
+                         void* workspace, size_t ws_bytes, int T, int H, float eps, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(dy, x, w, dres, dx, workspace);
+  const int nvec = H / 8;
+  if (H % 8 || nvec > 32 * 6 || T <= 0 || !dgamma || !dbeta || !dx) return DLLM_ERR_SHAPE;
+  if (ws_bytes < layernorm_bwd_affine_workspace(T, H)) return DLLM_ERR_SHAPE;
+  float2* stats = static_cast<float2*>(workspace);
+  float* partial = reinterpret_cast<float*>(static_cast<char*>(workspace) + static_cast<size_t>(T) * sizeof(float2));
+  const unsigned grid = static_cast<unsigned>((static_cast<long>(T) * 32 + 255) / 256);
+  if (nvec <= 64)
+    layernorm_bwd_warp_kernel<2, true><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps, stats);
+  else if (nvec <= 128)
+    layernorm_bwd_warp_kernel<4, true><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps, stats);
+  else
+    layernorm_bwd_warp_kernel<6, true><<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, (const bf16*)dres, (bf16*)dx, T, H, eps, stats);
+  layernorm_bwd_dwb_kernel<<<dim3((nvec + 31) / 32, kLnSplits), 256, 0, s>>>((const bf16*)dy, (const bf16*)x, stats, partial, T, H);
+  layernorm_dwb_final_kernel<<<(H + 255) / 256, 256, 0, s>>>(partial, (bf16*)dgamma, (bf16*)dbeta, H);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+
+// ---- Quick-GELU (CLIP MLP, transformers activations.QuickGELU) for the trainable tower, whose backward needs the pre-activation: fc1
+// runs as a bias-only GEMM and this kernel applies y = x * sigmoid(1.702 x) with the GEMM epilogue's formula (x / (1 + exp(-1.702 x))),
+// fp32, one rounding.  Backward: dx = dy * (s + 1.702 x s (1 - s)), s = sigmoid(1.702 x).  8 elements (one 16-byte vector) per thread.
+__global__ void quick_gelu_kernel(const V8* __restrict__ x, V8* __restrict__ y, long nvec) {
+  const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= nvec) return;
+  float f[8];
+  up8(x[i], f);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) f[j] = f[j] / (1.f + expf(-1.702f * f[j]));
+  y[i] = pk8(f);
+}
+__global__ void quick_gelu_bwd_kernel(const V8* __restrict__ dy, const V8* __restrict__ x, V8* __restrict__ dx, long nvec) {
+  const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= nvec) return;
+  float g[8], f[8];
+  up8(dy[i], g);
+  up8(x[i], f);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float sg = 1.f / (1.f + expf(-1.702f * f[j]));
+    g[j] = g[j] * (sg + 1.702f * f[j] * sg * (1.f - sg));
+  }
+  dx[i] = pk8(g);
+}
+int quick_gelu(const void* x, void* y, long n, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(x, y);
+  if (n <= 0 || n % 8 || !x || !y) return DLLM_ERR_SHAPE;
+  const long nvec = n / 8;
+  quick_gelu_kernel<<<static_cast<unsigned>((nvec + 255) / 256), 256, 0, s>>>((const V8*)x, (V8*)y, nvec);
+  return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
+}
+int quick_gelu_bwd(const void* dy, const void* x, void* dx, long n, cudaStream_t s) {
+  DLLM_REQUIRE_ALIGN16(dy, x, dx);
+  if (n <= 0 || n % 8 || !dy || !x || !dx) return DLLM_ERR_SHAPE;
+  const long nvec = n / 8;
+  quick_gelu_bwd_kernel<<<static_cast<unsigned>((nvec + 255) / 256), 256, 0, s>>>((const V8*)dy, (const V8*)x, (V8*)dx, nvec);
   return cudaGetLastError() == cudaSuccess ? 0 : DLLM_ERR_LAUNCH;
 }
 

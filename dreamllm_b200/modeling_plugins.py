@@ -171,9 +171,6 @@ class CLIPVisionEmbedding(MultimodalEmbedding):
         self.freeze_projector = freeze_projector
         if use_additional_post_layernorm:
             raise ValueError("use_additional_post_layernorm=True is not used by any shipped config and is not built")
-        if not freeze_clip_vision_model:
-            raise ValueError("the native CLIP tower is forward-only: freeze_clip_vision_model must be True "
-                             "(projects/dreamllm/configs/common.py:35)")
 
         src = clip_vision_model_name_or_path
         if isinstance(src, str):
@@ -198,7 +195,17 @@ class CLIPVisionEmbedding(MultimodalEmbedding):
         if pretrained_model_name_or_path is not None:
             self.load_model(pretrained_model_name_or_path)
         self.projector.load_model(projector_name_or_path)
-        self.clip_vision_model.requires_grad_(False)
+        # the reference's trainable set (modeling_plugins.py:248-257): with the tower unfrozen, post_layernorm and — for a negative
+        # select_layer — the layers after the selected hidden state stay frozen; the embeddings follow their own flag either way.  With
+        # select_layer >= 0 the layers at or past it keep requires_grad=True as there, although the tower never computes them: the
+        # gradient reducer and the sharded optimizer count their missing gradient as zero.
+        vm = self.clip_vision_model.vision_model
+        self.clip_vision_model.requires_grad_(not freeze_clip_vision_model)
+        if not freeze_clip_vision_model:
+            for i in range(select_layer + 1, 0):
+                vm.encoder.layers[i].requires_grad_(False)
+            vm.post_layernorm.requires_grad_(False)
+        vm.embeddings.requires_grad_(not freeze_embedding_layers)
         self.projector.requires_grad_(not freeze_projector)
 
     @property
@@ -226,7 +233,7 @@ class CLIPVisionEmbedding(MultimodalEmbedding):
                     freeze_embedding_layers=self.freeze_embedding_layers, freeze_projector=self.freeze_projector)
 
     def fsdp_ignored_modules(self) -> list:
-        out = [self.clip_vision_model]
+        out = [self.clip_vision_model] if self.freeze_clip_vision_model else []
         if self.freeze_projector:
             out.append(self.projector)
         return out

@@ -539,6 +539,52 @@ def layernorm_bwd(dy2d, x2d, weight, eps, dres=None):
     return dx
 
 
+def layernorm_bwd_affine(dy2d, x2d, weight, eps, dres=None, dgamma=None, dbeta=None):
+    """LayerNorm backward with the affine gradients: returns (dx, dgamma, dbeta).  dx (+ dres) has the bits of `layernorm_bwd`;
+    dgamma / dbeta are fp32 sums over the rows (order-fixed, no atomics) written as bf16 into `dgamma` / `dbeta` when given (e.g. the
+    parameters' gradient-bucket slices), else into new tensors."""
+    for t in (dy2d, x2d, weight, dres, dgamma, dbeta):
+        if t is not None and t.dtype != BF16:
+            raise TypeError(f"layernorm_bwd_affine takes bf16 tensors, got {t.dtype}")
+    _chk_cuda(dy2d, x2d, weight, dres, dgamma, dbeta)
+    T, H = x2d.shape
+    assert dy2d.shape == x2d.shape and dy2d.is_contiguous() and x2d.is_contiguous() and (dres is None or dres.is_contiguous())
+    dx = torch.empty_like(x2d)
+    dgamma = torch.empty(H, device=x2d.device, dtype=BF16) if dgamma is None else dgamma
+    dbeta = torch.empty(H, device=x2d.device, dtype=BF16) if dbeta is None else dbeta
+    assert dgamma.numel() == H and dbeta.numel() == H and dgamma.is_contiguous() and dbeta.is_contiguous()
+    wsb = lib().dllm_layernorm_bwd_affine_workspace_bytes(T, H)
+    ws = torch.empty(wsb, device=x2d.device, dtype=torch.uint8)
+    check(lib().dllm_layernorm_bwd_affine(_p(dy2d), _p(x2d), _p(weight), _p(dres), _p(dx), _p(dgamma), _p(dbeta), _p(ws), wsb, T, H,
+                                          float(eps), _stream()), "dllm_layernorm_bwd_affine")
+    LAUNCHES.add(3)
+    return dx, dgamma, dbeta
+
+
+def quick_gelu(x):
+    """y = x * sigmoid(1.702 x), bf16 (the fused GEMM epilogue's formula as a separate pass: the trainable CLIP tower keeps fc1's output)."""
+    if x.dtype != BF16:
+        raise TypeError(f"quick_gelu takes bf16, got {x.dtype}")
+    _chk_cuda(x)
+    assert x.is_contiguous()
+    y = torch.empty_like(x)
+    check(lib().dllm_quick_gelu(_p(x), _p(y), x.numel(), _stream()), "dllm_quick_gelu")
+    LAUNCHES.add(1)
+    return y
+
+
+def quick_gelu_bwd(dy, x):
+    """dx = dy * quick_gelu'(x), x the pre-activation."""
+    if dy.dtype != BF16 or x.dtype != BF16:
+        raise TypeError(f"quick_gelu_bwd takes bf16, got {dy.dtype} and {x.dtype}")
+    _chk_cuda(dy, x)
+    assert dy.is_contiguous() and x.is_contiguous() and dy.shape == x.shape
+    dx = torch.empty_like(x)
+    check(lib().dllm_quick_gelu_bwd(_p(dy), _p(x), _p(dx), x.numel(), _stream()), "dllm_quick_gelu_bwd")
+    LAUNCHES.add(1)
+    return dx
+
+
 def geglu_bwd(dout2d, in2d):
     _chk_cuda(dout2d, in2d)
     T, I2 = in2d.shape

@@ -217,6 +217,19 @@ int dllm_groupnorm_apply(const void* x, const void* w, const void* b, const floa
 int dllm_groupnorm_bwd_nhwc(const void* dy, const void* x, const void* w, const void* b, const float* stats, const void* dres, void* dx,
                             void* workspace, size_t ws_bytes, int N, int HW, int C, int G, int silu, void* stream);
 int dllm_layernorm_bwd(const void* dy, const void* x, const void* w, const void* dres, void* dx, int T, int H, float eps, void* stream);
+/* ---- CLIP vision tower training (freeze_clip_vision_model=False / freeze_embedding_layers=False, modeling_plugins.py:248-257) ----
+ * LayerNorm backward with the affine gradients: dx (+ dres) exactly as dllm_layernorm_bwd computes it (same bits), and
+ * dgamma[h] = sum_t dy[t, h] * xhat[t, h], dbeta[h] = sum_t dy[t, h] in fp32, written as bf16.  The sums are per-CTA fp32 partials in the
+ * caller's workspace (>= dllm_layernorm_bwd_affine_workspace_bytes(T, H)), added in a fixed order: no atomics, the bits depend only on
+ * the inputs and (T, H).  H % 8 == 0, H <= 1536; dy, x, w, dres, dx and the workspace 16-byte aligned (dgamma / dbeta are written
+ * element by element). */
+size_t dllm_layernorm_bwd_affine_workspace_bytes(int T, int H);
+int dllm_layernorm_bwd_affine(const void* dy, const void* x, const void* w, const void* dres, void* dx, void* dgamma, void* dbeta,
+                              void* workspace, size_t workspace_bytes, int T, int H, float eps, void* stream);
+/* y = x * sigmoid(1.702 x) (transformers QuickGELU) and dx = dy * (s + 1.702 x s (1 - s)), s = sigmoid(1.702 x): bf16 in and out, fp32
+ * arithmetic, one rounding, n % 8 == 0, 16-byte aligned pointers.  The forward uses the fused GEMM epilogue's formula. */
+int dllm_quick_gelu(const void* x, void* y, long n, void* stream);
+int dllm_quick_gelu_bwd(const void* dy, const void* x, void* dx, long n, void* stream);
 int dllm_geglu_bwd(const void* dout, const void* in, void* din, int T, int I, void* stream);
 int dllm_upsample2x_bwd_nhwc(const void* dy, void* dx, int N, int H, int W, int C, void* stream);
 int dllm_col2im_s2_nhwc(const void* dcols, void* dx, int N, int H, int W, int C, void* stream);
