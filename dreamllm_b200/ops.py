@@ -158,17 +158,16 @@ def linear(x2d: torch.Tensor, weight: torch.Tensor, out=None, out_dtype=BF16, bi
     return gemm(x2d, weight, out=out, out_dtype=out_dtype, bias=bias, residual=residual, act=act)
 
 
-def geglu_permute(weight: torch.Tensor, bias: torch.Tensor | None):
-    """`GEGLU.proj` weight [2I, K] / bias [2I] -> row order [64 value rows | their 64 gate rows] per 128-row group (what `linear_geglu`
-    expects).  I % 64 == 0."""
-    I2, K = weight.shape
-    inner = I2 // 2
+def _geglu_rows(t: torch.Tensor) -> torch.Tensor:
+    """[2I, ...] -> row order [64 value rows | their 64 gate rows] per 128-row group.  I % 64 == 0."""
+    inner = t.shape[0] // 2
     assert inner % 64 == 0
-    wp = torch.stack([weight[:inner].view(inner // 64, 64, K), weight[inner:].view(inner // 64, 64, K)], dim=1).reshape(I2, K).contiguous()
-    bp = None
-    if bias is not None:
-        bp = torch.stack([bias[:inner].view(inner // 64, 64), bias[inner:].view(inner // 64, 64)], dim=1).reshape(I2).contiguous()
-    return wp, bp
+    return t.view(2, inner // 64, 64, *t.shape[1:]).transpose(0, 1).reshape(t.shape).contiguous()
+
+
+def geglu_permute(weight: torch.Tensor, bias: torch.Tensor | None):
+    """`GEGLU.proj` weight [2I, K] / bias [2I] -> the row order `linear_geglu` expects."""
+    return _geglu_rows(weight), None if bias is None else _geglu_rows(bias)
 
 
 def linear_geglu(x2d: torch.Tensor, w_perm: torch.Tensor, b_perm: torch.Tensor | None) -> torch.Tensor:
@@ -461,11 +460,6 @@ def zero_rows_(dst2d, idx):
 
 
 # ----------------------------------------------------------------------------------------------- UNet ops (NHWC bf16)
-def attn_fwd_cross(q, k, v, scale=None):
-    """q [B,Sq,nh,d], k/v [B,Skv,nkv,d] (views; k and v share a token stride; nkv divides nh). Non-causal. returns out [B,Sq,nh*d]."""
-    return attn_fwd_cross_lse(q, k, v, scale)[0]
-
-
 def conv3x3(x_nhwc, w_k, bias=None, rowbias=None, residual=None):
     """x [N,H,W,Cin] bf16 contiguous; w_k [Cout, 9*Cin] ((r,s,c)-major); returns [N,H,W,Cout]."""
     _chk_cuda(x_nhwc, w_k, bias, rowbias, residual)
@@ -612,6 +606,8 @@ def attn_bwd_cross(dout, q, k, v, out, lse, dq, dk, dv, scale=None):
 
 
 def attn_fwd_cross_lse(q, k, v, scale=None):
+    """q [B,Sq,nh,d], k/v [B,Skv,nkv,d] (views; k and v share a token stride; nkv divides nh). Non-causal.
+    Returns (out [B,Sq,nh*d], lse [B,nh,Sq] fp32)."""
     _chk_cuda(q, k, v)
     B, Sq, nh, d = q.shape
     Skv, nkv = k.shape[1], _kv_heads(q, k)
@@ -774,6 +770,23 @@ def _cached_weight(key, w, build):
             ent = (tag, build(w.detach()), weakref.ref(w, lambda _r, _k=key: _WCACHE.pop(_k, None)))
         _WCACHE[key] = ent
     return ent[1]
+
+
+def conv3x3_weight(weight):
+    """Conv2d weight [Cout, Cin, 3, 3] -> [Cout, 9*Cin] with k = (r, s, c): the implicit-GEMM / im2col K order of `conv3x3` and
+    `im2col_s2`."""
+    return _cached_weight(("conv3x3", id(weight)), weight, lambda w: w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous())
+
+
+def conv3x3_dgrad_weight(weight):
+    """w2[ci, r', s', co] = w[co, ci, 2-r', 2-s'] as [Cin, 9*Cout]: dgrad(x) = conv3x3(dy, w2)."""
+    return _cached_weight(("conv3x3_dgrad", id(weight)), weight,
+                          lambda w: w.flip(2, 3).permute(1, 2, 3, 0).reshape(w.shape[1], -1).contiguous())
+
+
+def geglu_weights(weight, bias):
+    """`geglu_permute(weight, bias)`, cached: each of the two is rebuilt when its own parameter changes."""
+    return (_cached_weight(("geglu_w", id(weight)), weight, _geglu_rows), _cached_weight(("geglu_b", id(bias)), bias, _geglu_rows))
 
 
 def conv_in(latents_nchw_f32, weight, bias, batch_out):

@@ -171,19 +171,6 @@ class UNet2DConditionModel(nn.Module):
             self.up_blocks.append(b)
         self.conv_norm_out = nn.GroupNorm(G, ch[0], eps=eps)
         self.conv_out = nn.Conv2d(ch[0], c["out_channels"], 3, padding=1)
-        self._wcache = {}
-
-    # ---- weight layout caches (frozen tower: built once) ----
-    def _conv_w(self, conv: nn.Conv2d):
-        """[Cout, Cin, 3, 3] -> [Cout, 9*Cin] with k = (r, s, c): the implicit-GEMM / im2col K order."""
-        key = id(conv)
-        w = conv.weight
-        ent = self._wcache.get(key)
-        if ent is None or ent[0] != (w.data_ptr(), w._version):
-            wk = w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
-            ent = ((w.data_ptr(), w._version), wk)
-            self._wcache[key] = ent
-        return ent[1]
 
     def transformers(self):
         for b in list(self.down_blocks) + [self.mid_block] + list(self.up_blocks):
@@ -241,63 +228,118 @@ class UNet2DConditionModel(nn.Module):
         temb = ops.linear(t1, te.linear_2.weight, bias=te.linear_2.bias, residual=aug_emb)     # the epilogue adds residual after act
         return temb, ops.silu(temb)
 
-    # ---- building blocks (x: NHWC bf16) ----
-    def _resnet(self, r: ResnetBlock2D, x, temb_act):
-        N, H, W, Cin = x.shape
+    # ---- the forward (x: NHWC bf16), one walk for the sampler (tape None) and the training pass (tape: a list) ----
+    # The training pass appends what `backward_cond` replays in reverse to `tape` and runs FF-in as Linear + GEGLU to keep the projection;
+    # the sampler keeps nothing and fuses GEGLU into the FF-in epilogue (same bits).  The `del`s free what the sampler no longer needs: its
+    # captured graph's memory pool is as large as the most activations alive at once.
+    def _groupnorm(self, norm: nn.GroupNorm, x, silu, tape):
+        """-> (y, stats [N, G, 2] for the backward, or None without a tape); both forms run the same three kernels."""
         G = self.cfg["norm_num_groups"]
-        h = ops.groupnorm(x, r.norm1.weight, r.norm1.bias, G, r.norm1.eps, silu=True)
+        if tape is None:
+            return ops.groupnorm(x, norm.weight, norm.bias, G, norm.eps, silu=silu), None
+        return ops.groupnorm(x, norm.weight, norm.bias, G, norm.eps, silu=silu, return_stats=True)
+
+    def _resnet(self, r: ResnetBlock2D, x, temb_act, tape):
+        N, H, W, Cin = x.shape
+        h, st1 = self._groupnorm(r.norm1, x, True, tape)
         rowb = ops.linear(temb_act, r.time_emb_proj.weight, bias=r.time_emb_proj.bias)            # [N, Cout]
-        h = ops.conv3x3(h, self._conv_w(r.conv1), bias=r.conv1.bias, rowbias=rowb)
-        h = ops.groupnorm(h, r.norm2.weight, r.norm2.bias, G, r.norm2.eps, silu=True)
+        c1 = ops.conv3x3(h, ops.conv3x3_weight(r.conv1.weight), bias=r.conv1.bias, rowbias=rowb)
+        del h
+        h, st2 = self._groupnorm(r.norm2, c1, True, tape)
+        if tape is not None:
+            tape.append(("res", r, x, st1, c1, st2))
+        del c1
         if r.conv_shortcut is None:
             sc = x
         else:
             wsc = r.conv_shortcut.weight.view(r.conv_shortcut.weight.shape[0], Cin)
             sc = ops.linear(x.view(-1, Cin), wsc, bias=r.conv_shortcut.bias).view(N, H, W, -1)
-        return ops.conv3x3(h, self._conv_w(r.conv2), bias=r.conv2.bias, residual=sc)
+        return ops.conv3x3(h, ops.conv3x3_weight(r.conv2.weight), bias=r.conv2.bias, residual=sc)
 
-    def _transformer(self, t: Transformer2DModel, x, kv):
+    def _transformer(self, t: Transformer2DModel, x, kv, tape):
         """kv: iterator over the per-block cross K/V tensors of `precompute_cross_kv` (one per BasicTransformerBlock)."""
         N, H, W, C = x.shape
         T = N * H * W
-        x2 = x.view(T, C)
-        h = ops.groupnorm(x, t.norm.weight, t.norm.bias, self.cfg["norm_num_groups"], t.norm.eps, silu=False).view(T, C)
-        h = ops.linear(h, t.proj_in.weight, bias=t.proj_in.bias)
+        h, st = self._groupnorm(t.norm, x, False, tape)
+        h = ops.linear(h.view(T, C), t.proj_in.weight, bias=t.proj_in.bias)
+        saved = None if tape is None else []
         for blk in t.transformer_blocks:
-            h = self._block(blk, h, next(kv), N, H * W)
-        return ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
+            h = self._block(blk, h, next(kv), N, H * W, saved)
+        out = ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x.view(T, C)).view(N, H, W, C)
+        if tape is not None:
+            tape.append(("tr", t, x, st, saved))
+        return out
 
-    def _block(self, blk: BasicTransformerBlock, h, ctx_kv, N, S):
-        T, C = h.shape
+    def _block(self, blk: BasicTransformerBlock, h0, ctx_kv, N, S, saved):
+        T, C = h0.shape
         nh = blk.attn1.heads
         # self-attention
-        y = ops.layernorm_fwd(h, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
+        y = ops.layernorm_fwd(h0, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
         wqkv = _fuse_rows([blk.attn1.to_q.weight, blk.attn1.to_k.weight, blk.attn1.to_v.weight])
         qkv = ops.linear(y, wqkv).view(N, S, 3, nh, 64)
-        ao, _ = ops.attn_fwd(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal=False)
-        h = ops.linear(ao.view(T, C), blk.attn1.to_out[0].weight, bias=blk.attn1.to_out[0].bias, residual=h)
+        ao1, lse1 = ops.attn_fwd(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal=False)
+        h1 = ops.linear(ao1.view(T, C), blk.attn1.to_out[0].weight, bias=blk.attn1.to_out[0].bias, residual=h0)
         # cross-attention on the dream-query conditioning (K/V precomputed per prompt)
-        y = ops.layernorm_fwd(h, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
-        q = ops.linear(y, blk.attn2.to_q.weight).view(N, S, nh, 64)
-        Q = ctx_kv.shape[1]
-        kv = ctx_kv.view(N, Q, 2, nh, 64)
-        ao = ops.attn_fwd_cross(q, kv[:, :, 0], kv[:, :, 1])
-        h = ops.linear(ao.view(T, C), blk.attn2.to_out[0].weight, bias=blk.attn2.to_out[0].bias, residual=h)
+        y = ops.layernorm_fwd(h1, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
+        q2 = ops.linear(y, blk.attn2.to_q.weight).view(N, S, nh, 64)
+        kv = ctx_kv.view(N, ctx_kv.shape[1], 2, nh, 64)
+        ao2, lse2 = ops.attn_fwd_cross_lse(q2, kv[:, :, 0], kv[:, :, 1])
+        if saved is None:
+            del lse2, ao1
+        h2 = ops.linear(ao2.view(T, C), blk.attn2.to_out[0].weight, bias=blk.attn2.to_out[0].bias, residual=h1)
+        if saved is None:
+            del h1
         # GEGLU feed-forward
-        y = ops.layernorm_fwd(h, blk.norm3.weight, blk.norm3.bias, blk.norm3.eps)
-        g = ops.linear_geglu(y, *self._geglu_w(blk.ff.net[0].proj))       # FF-in GEMM with h * gelu(gate) in its epilogue
-        return ops.linear(g, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h)
+        y = ops.layernorm_fwd(h2, blk.norm3.weight, blk.norm3.bias, blk.norm3.eps)
+        proj = blk.ff.net[0].proj
+        if saved is None:
+            g = ops.linear_geglu(y, *ops.geglu_weights(proj.weight, proj.bias))       # FF-in GEMM with h * gelu(gate) in its epilogue
+        else:
+            f = ops.linear(y, proj.weight, bias=proj.bias)
+            g = ops.geglu(f)
+            saved.append((blk, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f))
+        return ops.linear(g, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h2)
 
-    def _geglu_w(self, proj: nn.Linear):
-        """Row-permuted copy of `GEGLU.proj` ([64 value | 64 gate] per 128 rows) for the fused epilogue; the parameter itself keeps the
-        diffusers layout (state-dict compatible).  Frozen tower: built once."""
-        key = ("geglu", id(proj))
-        w = proj.weight
-        ent = self._wcache.get(key)
-        if ent is None or ent[0] != (w.data_ptr(), w._version):
-            ent = ((w.data_ptr(), w._version), ops.geglu_permute(w.detach(), proj.bias.detach()))
-            self._wcache[key] = ent
-        return ent[1]
+    def _walk(self, latents_nchw_f32, temb_act, cross_kv, batch, tape=None, eps_out=None):
+        """conv_in -> down / mid / up blocks -> conv_norm_out -> conv_out: eps [batch, 4, H, W] fp32."""
+        x = ops.conv_in(latents_nchw_f32, self.conv_in.weight, self.conv_in.bias, batch)
+        skips = [x]
+        kv = iter(cross_kv)
+        for b in self.down_blocks:
+            for j, r in enumerate(b.resnets):
+                x = self._resnet(r, x, temb_act, tape)
+                if hasattr(b, "attentions"):
+                    x = self._transformer(b.attentions[j], x, kv, tape)
+                skips.append(x)
+                if tape is not None:
+                    tape.append(("skip_push",))
+            if hasattr(b, "downsamplers"):
+                conv = b.downsamplers[0].conv
+                N, H, W, C = x.shape
+                x = ops.linear(ops.im2col_s2(x), ops.conv3x3_weight(conv.weight), bias=conv.bias).view(N, H // 2, W // 2, -1)
+                skips.append(x)
+                if tape is not None:
+                    tape.extend([("down", conv, (N, H, W, C)), ("skip_push",)])
+        x = self._resnet(self.mid_block.resnets[0], x, temb_act, tape)
+        x = self._transformer(self.mid_block.attentions[0], x, kv, tape)
+        x = self._resnet(self.mid_block.resnets[1], x, temb_act, tape)
+        for b in self.up_blocks:
+            for j, r in enumerate(b.resnets):
+                if tape is not None:
+                    tape.append(("cat", x.shape[-1]))
+                x = self._resnet(r, ops.concat_channels(x, skips.pop()), temb_act, tape)
+                if hasattr(b, "attentions"):
+                    x = self._transformer(b.attentions[j], x, kv, tape)
+            if hasattr(b, "upsamplers"):
+                conv = b.upsamplers[0].conv
+                x = ops.conv3x3(ops.upsample2x(x), ops.conv3x3_weight(conv.weight), bias=conv.bias)
+                if tape is not None:
+                    tape.append(("up", conv))
+        xn, stn = self._groupnorm(self.conv_norm_out, x, True, tape)
+        if tape is not None:
+            tape.append(("out", x, stn))
+        del x
+        return ops.conv_out(xn, self.conv_out.weight, self.conv_out.bias, out=eps_out)
 
     @torch.no_grad()
     def precompute_cross_kv(self, encoder_hidden_states):
@@ -316,118 +358,30 @@ class UNet2DConditionModel(nn.Module):
         """latents [Bl,4,H,W] fp32 (Bl divides batch: CFG duplication); temb_sin [batch, 320] bf16 sinusoidal embedding;
         cross_kv from `precompute_cross_kv`; aug_emb [batch, 1280] bf16 from `add_embedding_fwd` (SDXL only) -> eps [batch,4,H,W] fp32."""
         _, temb_act = self._temb_act(temb_sin, aug_emb)          # silu(temb): all the resnets read
-        x = ops.conv_in(latents_nchw_f32, self.conv_in.weight, self.conv_in.bias, batch)
-        skips = [x]
-        kv = iter(cross_kv)
-        for b in self.down_blocks:
-            for j, r in enumerate(b.resnets):
-                x = self._resnet(r, x, temb_act)
-                if hasattr(b, "attentions"):
-                    x = self._transformer(b.attentions[j], x, kv)
-                skips.append(x)
-            if hasattr(b, "downsamplers"):
-                conv = b.downsamplers[0].conv
-                N, H, W, C = x.shape
-                cols = ops.im2col_s2(x)
-                x = ops.linear(cols, self._conv_w(conv), bias=conv.bias).view(N, H // 2, W // 2, -1)
-                skips.append(x)
-        x = self._resnet(self.mid_block.resnets[0], x, temb_act)
-        x = self._transformer(self.mid_block.attentions[0], x, kv)
-        x = self._resnet(self.mid_block.resnets[1], x, temb_act)
-        for b in self.up_blocks:
-            for j, r in enumerate(b.resnets):
-                x = self._resnet(r, ops.concat_channels(x, skips.pop()), temb_act)
-                if hasattr(b, "attentions"):
-                    x = self._transformer(b.attentions[j], x, kv)
-            if hasattr(b, "upsamplers"):
-                conv = b.upsamplers[0].conv
-                x = ops.conv3x3(ops.upsample2x(x), self._conv_w(conv), bias=conv.bias)
-        x = ops.groupnorm(x, self.conv_norm_out.weight, self.conv_norm_out.bias, self.cfg["norm_num_groups"], self.conv_norm_out.eps, silu=True)
-        return ops.conv_out(x, self.conv_out.weight, self.conv_out.bias, out=eps_out)
-
+        return self._walk(latents_nchw_f32, temb_act, cross_kv, batch, eps_out=eps_out)
 
     # ================================================================================================ training path
     # StableDiffusionHead.forward (modeling_plugins.py:493-577) back-propagates through the FROZEN UNet into the dream-query
     # conditioning.  `forward_train` is the same forward with a tape; `backward_cond` walks it in reverse computing input
     # gradients only (conv dgrad = implicit-GEMM conv with the flipped/transposed filter, Linear dgrad = NN GEMM, GroupNorm /
     # LayerNorm / GEGLU / attention backward kernels) and returns d(loss)/d(encoder_hidden_states).
-    def _conv_w_dgrad(self, conv: nn.Conv2d):
-        """w2[ci, r', s', co] = w[co, ci, 2-r', 2-s'] as [Cin, 9*Cout]: dgrad(x) = conv3x3(dy, w2)."""
-        key = ("dg", id(conv))
-        w = conv.weight
-        ent = self._wcache.get(key)
-        if ent is None or ent[0] != (w.data_ptr(), w._version):
-            wk = w.detach().flip(2, 3).permute(1, 2, 3, 0).reshape(w.shape[1], -1).contiguous()
-            ent = ((w.data_ptr(), w._version), wk)
-            self._wcache[key] = ent
-        return ent[1]
-
-    def _resnet_fwd(self, r, x, temb_act, tape):
-        N, H, W, Cin = x.shape
-        G = self.cfg["norm_num_groups"]
-        h, st1 = ops.groupnorm(x, r.norm1.weight, r.norm1.bias, G, r.norm1.eps, silu=True, return_stats=True)
-        rowb = ops.linear(temb_act, r.time_emb_proj.weight, bias=r.time_emb_proj.bias)
-        c1 = ops.conv3x3(h, self._conv_w(r.conv1), bias=r.conv1.bias, rowbias=rowb)
-        h, st2 = ops.groupnorm(c1, r.norm2.weight, r.norm2.bias, G, r.norm2.eps, silu=True, return_stats=True)
-        if r.conv_shortcut is None:
-            sc = x
-        else:
-            sc = ops.linear(x.view(-1, Cin), r.conv_shortcut.weight.view(-1, Cin), bias=r.conv_shortcut.bias).view(N, H, W, -1)
-        out = ops.conv3x3(h, self._conv_w(r.conv2), bias=r.conv2.bias, residual=sc)
-        tape.append(("res", r, x, st1, c1, st2))
-        return out
-
     def _resnet_bwd(self, ent, dout, drowb=None):
         """drowb: {resnet: [N, Cout] bf16 column slice} when the time embedding needs a gradient (SDXL); the resnet's time_emb_proj
         output gradient, sum over pixels of d(conv1 output), is written there."""
         _, r, x, st1, c1, st2 = ent
         N, H, W, Cin = x.shape
         G = self.cfg["norm_num_groups"]
-        dh2 = ops.conv3x3(dout, self._conv_w_dgrad(r.conv2))
+        dh2 = ops.conv3x3(dout, ops.conv3x3_dgrad_weight(r.conv2.weight))
         dc1 = ops.groupnorm_bwd(dh2, c1, r.norm2.weight, r.norm2.bias, st2, G, True)
         if drowb is not None:
             ops.channel_sum_nhwc(dc1, out=drowb[r])
-        dh1 = ops.conv3x3(dc1, self._conv_w_dgrad(r.conv1))
+        dh1 = ops.conv3x3(dc1, ops.conv3x3_dgrad_weight(r.conv1.weight))
         if r.conv_shortcut is None:
             dsc = dout
         else:
             Cout = dout.shape[-1]
             dsc = ops.linear_dgrad(dout.view(-1, Cout), r.conv_shortcut.weight.view(Cout, Cin)).view(N, H, W, Cin)
         return ops.groupnorm_bwd(dh1, x, r.norm1.weight, r.norm1.bias, st1, G, True, dres=dsc)
-
-    def _transformer_fwd(self, t, x, kv, tape):
-        N, H, W, C = x.shape
-        T, S = N * H * W, H * W
-        x2 = x.view(T, C)
-        g, st = ops.groupnorm(x, t.norm.weight, t.norm.bias, self.cfg["norm_num_groups"], t.norm.eps, silu=False, return_stats=True)
-        h = ops.linear(g.view(T, C), t.proj_in.weight, bias=t.proj_in.bias)
-        saved = []
-        for blk in t.transformer_blocks:
-            h = self._block_fwd(blk, h, next(kv), N, S, saved)
-        out = ops.linear(h, t.proj_out.weight, bias=t.proj_out.bias, residual=x2).view(N, H, W, C)
-        tape.append(("tr", t, x, st, saved))
-        return out
-
-    def _block_fwd(self, blk, h0, ctx_kv, N, S, saved):
-        T, C = h0.shape
-        nh = blk.attn1.heads
-        y = ops.layernorm_fwd(h0, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
-        wqkv = _fuse_rows([blk.attn1.to_q.weight, blk.attn1.to_k.weight, blk.attn1.to_v.weight])
-        qkv = ops.linear(y, wqkv).view(N, S, 3, nh, 64)
-        ao1, lse1 = ops.attn_fwd(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal=False)
-        h1 = ops.linear(ao1.view(T, C), blk.attn1.to_out[0].weight, bias=blk.attn1.to_out[0].bias, residual=h0)
-        y = ops.layernorm_fwd(h1, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
-        q2 = ops.linear(y, blk.attn2.to_q.weight).view(N, S, nh, 64)
-        Q = ctx_kv.shape[1]
-        kv = ctx_kv.view(N, Q, 2, nh, 64)
-        ao2, lse2 = ops.attn_fwd_cross_lse(q2, kv[:, :, 0], kv[:, :, 1])
-        h2 = ops.linear(ao2.view(T, C), blk.attn2.to_out[0].weight, bias=blk.attn2.to_out[0].bias, residual=h1)
-        y = ops.layernorm_fwd(h2, blk.norm3.weight, blk.norm3.bias, blk.norm3.eps)
-        f = ops.linear(y, blk.ff.net[0].proj.weight, bias=blk.ff.net[0].proj.bias)
-        gg = ops.geglu(f)
-        h3 = ops.linear(gg, blk.ff.net[2].weight, bias=blk.ff.net[2].bias, residual=h2)
-        saved.append((blk, h0, qkv, ao1, lse1, h1, q2, ctx_kv, ao2, lse2, h2, f))
-        return h3
 
     def _transformer_bwd(self, ent, dout, dkv_list):
         _, t, x, st, saved = ent
@@ -473,13 +427,7 @@ class UNet2DConditionModel(nn.Module):
         added_cond = (text_embeds [B, 1280], time_ids [B, 6]) for an SDXL UNet: the tape then also keeps what the gradient into
         text_embeds (through add_embedding and every resnet's time_emb_proj) needs."""
         B = latents_nchw_f32.shape[0]
-        tape = []
-        cond2 = encoder_hidden_states.to(BF16).reshape(-1, encoder_hidden_states.shape[-1]).contiguous()
-        Q = encoder_hidden_states.shape[1]
-        kvs = []
-        for blk in self.blocks():
-            a = blk.attn2
-            kvs.append(ops.linear(cond2, _fuse_rows([a.to_k.weight, a.to_v.weight])).view(B, Q, -1))
+        kvs = self.precompute_cross_kv(encoder_hidden_states)
         temb_sin = ops.timestep_embedding_batch(t_i32, self.cfg["block_out_channels"][0])
         xl = None
         aug = None
@@ -492,42 +440,9 @@ class UNet2DConditionModel(nn.Module):
         temb, temb_act = self._temb_act(temb_sin, aug)
         if xl is not None:
             xl["temb"] = temb
-        x = ops.conv_in(latents_nchw_f32, self.conv_in.weight, self.conv_in.bias, B)
-        skips = [x]
-        kv = iter(kvs)
-        for b in self.down_blocks:
-            for j, r in enumerate(b.resnets):
-                x = self._resnet_fwd(r, x, temb_act, tape)
-                if hasattr(b, "attentions"):
-                    x = self._transformer_fwd(b.attentions[j], x, kv, tape)
-                skips.append(x)
-                tape.append(("skip_push",))
-            if hasattr(b, "downsamplers"):
-                conv = b.downsamplers[0].conv
-                N, H, W, C = x.shape
-                x = ops.linear(ops.im2col_s2(x), self._conv_w(conv), bias=conv.bias).view(N, H // 2, W // 2, -1)
-                tape.append(("down", conv, (N, H, W, C)))
-                skips.append(x)
-                tape.append(("skip_push",))
-        x = self._resnet_fwd(self.mid_block.resnets[0], x, temb_act, tape)
-        x = self._transformer_fwd(self.mid_block.attentions[0], x, kv, tape)
-        x = self._resnet_fwd(self.mid_block.resnets[1], x, temb_act, tape)
-        for b in self.up_blocks:
-            for j, r in enumerate(b.resnets):
-                sk = skips.pop()
-                tape.append(("cat", x.shape[-1]))
-                x = self._resnet_fwd(r, ops.concat_channels(x, sk), temb_act, tape)
-                if hasattr(b, "attentions"):
-                    x = self._transformer_fwd(b.attentions[j], x, kv, tape)
-            if hasattr(b, "upsamplers"):
-                conv = b.upsamplers[0].conv
-                x = ops.conv3x3(ops.upsample2x(x), self._conv_w(conv), bias=conv.bias)
-                tape.append(("up", conv))
-        xn, stn = ops.groupnorm(x, self.conv_norm_out.weight, self.conv_norm_out.bias, self.cfg["norm_num_groups"], self.conv_norm_out.eps,
-                               silu=True, return_stats=True)
-        tape.append(("out", x, stn))
-        eps = ops.conv_out(xn, self.conv_out.weight, self.conv_out.bias)
-        return eps, (tape, B, Q, xl)
+        tape = []
+        eps = self._walk(latents_nchw_f32, temb_act, kvs, B, tape=tape)
+        return eps, (tape, B, encoder_hidden_states.shape[1], xl)
 
     def backward_cond(self, deps_nchw_f32, tape_pack):
         """d(loss)/d(eps) [B,4,H,W] fp32 -> d(loss)/d(encoder_hidden_states) [B,Q,ctx] bf16; for a tape recorded with `added_cond`,
@@ -557,7 +472,7 @@ class UNet2DConditionModel(nn.Module):
             elif kind == "tr":
                 dx = self._transformer_bwd(ent, dx, dkv_list)
             elif kind == "up":
-                dx = ops.upsample2x_bwd(ops.conv3x3(dx, self._conv_w_dgrad(ent[1])))
+                dx = ops.upsample2x_bwd(ops.conv3x3(dx, ops.conv3x3_dgrad_weight(ent[1].weight)))
             elif kind == "cat":
                 dx, dsk = ops.split_channels(dx, ent[1])
                 skip_grads.append(dsk)
@@ -567,7 +482,7 @@ class UNet2DConditionModel(nn.Module):
             elif kind == "down":
                 conv, (N, H, W, C) = ent[1], ent[2]
                 Cout = dx.shape[-1]
-                dcols = ops.linear_dgrad(dx.reshape(-1, Cout), self._conv_w(conv))
+                dcols = ops.linear_dgrad(dx.reshape(-1, Cout), ops.conv3x3_weight(conv.weight))
                 dx = ops.col2im_s2(dcols, N, H, W, C)
             else:
                 raise RuntimeError(kind)

@@ -78,26 +78,16 @@ class AutoencoderKLEncoder(nn.Module):
         self.cfg = c
         self.encoder = Encoder(c)
         self.quant_conv = nn.Conv2d(2 * c["latent_channels"], 2 * c["latent_channels"], 1)
-        self._wcache = {}
-
-    def _conv_w(self, conv):
-        key = id(conv)
-        w = conv.weight
-        ent = self._wcache.get(key)
-        if ent is None or ent[0] != (w.data_ptr(), w._version):
-            ent = ((w.data_ptr(), w._version), w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous())
-            self._wcache[key] = ent
-        return ent[1]
 
     def _resnet(self, r, x):
         N, H, W, Cin = x.shape
         G = self.cfg["norm_num_groups"]
         h = ops.groupnorm(x, r.norm1.weight, r.norm1.bias, G, r.norm1.eps, silu=True)
-        h = ops.conv3x3(h, self._conv_w(r.conv1), bias=r.conv1.bias)
+        h = ops.conv3x3(h, ops.conv3x3_weight(r.conv1.weight), bias=r.conv1.bias)
         h = ops.groupnorm(h, r.norm2.weight, r.norm2.bias, G, r.norm2.eps, silu=True)
         sc = x if r.conv_shortcut is None else ops.linear(x.view(-1, Cin), r.conv_shortcut.weight.view(-1, Cin),
                                                          bias=r.conv_shortcut.bias).view(N, H, W, -1)
-        return ops.conv3x3(h, self._conv_w(r.conv2), bias=r.conv2.bias, residual=sc)
+        return ops.conv3x3(h, ops.conv3x3_weight(r.conv2.weight), bias=r.conv2.bias, residual=sc)
 
     def _attention(self, a, x):
         N, H, W, C = x.shape
@@ -127,7 +117,7 @@ class AutoencoderKLEncoder(nn.Module):
             if hasattr(b, "downsamplers"):
                 conv = b.downsamplers[0].conv
                 N, Hh, Ww, C = x.shape
-                x = ops.linear(ops.im2col_s2(x, pad=0), self._conv_w(conv), bias=conv.bias).view(N, Hh // 2, Ww // 2, -1)
+                x = ops.linear(ops.im2col_s2(x, pad=0), ops.conv3x3_weight(conv.weight), bias=conv.bias).view(N, Hh // 2, Ww // 2, -1)
         x = self._resnet(e.mid_block.resnets[0], x)
         x = self._attention(e.mid_block.attentions[0], x)
         x = self._resnet(e.mid_block.resnets[1], x)
@@ -179,7 +169,6 @@ class AutoencoderKLDecoder(AutoencoderKLEncoder):
         self.cfg = c
         self.decoder = Decoder(c)
         self.post_quant_conv = nn.Conv2d(c["latent_channels"], c["latent_channels"], 1)
-        self._wcache = {}
 
     @torch.no_grad()
     def decode(self, latents):
@@ -202,6 +191,6 @@ class AutoencoderKLDecoder(AutoencoderKLEncoder):
                 x = self._resnet(r, x)
             if hasattr(b, "upsamplers"):
                 conv = b.upsamplers[0].conv
-                x = ops.conv3x3(ops.upsample2x(x), self._conv_w(conv), bias=conv.bias)
+                x = ops.conv3x3(ops.upsample2x(x), ops.conv3x3_weight(conv.weight), bias=conv.bias)
         x = ops.groupnorm(x, d.conv_norm_out.weight, d.conv_norm_out.bias, self.cfg["norm_num_groups"], d.conv_norm_out.eps, silu=True)
         return ops.conv_out(x, d.conv_out.weight, d.conv_out.bias)

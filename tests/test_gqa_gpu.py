@@ -187,7 +187,7 @@ def test_gqa_rejects_heads_not_divisible():
     q = torch.zeros(1, 64, 6, 64, dtype=BF, device="cuda")
     k = torch.zeros(1, 64, 4, 64, dtype=BF, device="cuda")
     with pytest.raises(AssertionError, match="multiple of"):
-        ops.attn_fwd_cross(q, k, k)
+        ops.attn_fwd_cross_lse(q, k, k)
     from dreamllm_b200._lib import lib
     L = lib()
     out = torch.empty(1, 64, 6 * 64, dtype=BF, device="cuda")
