@@ -649,7 +649,7 @@ static SplitPlan plan_split(int M, int N, int K) {
   int slots = num_sms() - g_reserved_sms;
   if (slots < 1) slots = 1;
   int ks = 1;
-  if (tiles * 2 <= slots && num_kb >= 8) {
+  if (tiles > 0 && tiles * 2 <= slots && num_kb >= 8) {   // (an empty output plans no split: its entry points refuse the shape)
     ks = slots / tiles;
     if (ks > num_kb / 4) ks = num_kb / 4;    // at least 4 K blocks per slice
     if (ks > 16) ks = 16;
@@ -838,7 +838,7 @@ int conv3x3_nhwc(const void* x, const void* w, void* y, int Nimg, int H, int W, 
 // With a workspace of conv3x3_splitk_workspace() bytes small planes run split-K (see plan_split).
 int conv3x3_nhwc_ws(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const void* bias,
                     const void* rowbias, const void* residual, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  if (Nimg <= 0 || Cin % 64 || Cout % 8) return DLLM_ERR_SHAPE;
+  if (Nimg <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cin % 64 || Cout <= 0 || Cout % 8) return DLLM_ERR_SHAPE;
   if (W > 128 ? (W % 128) : (128 % W)) return DLLM_ERR_SHAPE;
   if (reinterpret_cast<uintptr_t>(y) & 1) return DLLM_ERR_ALIGN;
   const int HW = H * W;

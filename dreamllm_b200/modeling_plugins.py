@@ -661,6 +661,12 @@ class StableDiffusionHead(MultimodalHead):
         width = width or self.resolution
         if height % 8 or width % 8:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        planes = ops.diffusion_conv_planes(height, width, len(self.unet.cfg["block_out_channels"]),
+                                           len(self.vae_decoder.cfg["block_out_channels"]))
+        bad = [p for p in planes if not ops.conv3x3_plane_ok(*p)]
+        if bad:
+            raise ValueError(f"height x width = {height} x {width} is not supported: the UNet / VAE 3x3 convolutions would run on the "
+                             f"H x W planes {bad}, and each plane needs {ops.CONV3X3_PLANE_RULE}.")
         assert prompt_embeds is not None, "`prompt_embeds` must be provided by LLM."
         n_img = int(num_images_per_prompt or 1)
         if n_img > 1:                                           # (:760-772) each prompt's embeddings repeated per requested image

@@ -460,6 +460,35 @@ def zero_rows_(dst2d, idx):
 
 
 # ----------------------------------------------------------------------------------------------- UNet ops (NHWC bf16)
+CONV3X3_PLANE_RULE = ("W a multiple of 128, or W dividing 128 with H a multiple of 128 / W, or H dividing 128 / W "
+                      "(a tile of several whole images)")
+
+
+def conv3x3_plane_ok(H: int, W: int) -> bool:
+    """Whether `conv3x3` takes an H x W plane: each 128-pixel tile is one TMA box of whole rows of whole images, or a 128-column piece
+    of a row (the plane rule of dllm_conv3x3_nhwc_ws)."""
+    if H <= 0 or W <= 0:
+        return False
+    if W > 128:
+        return W % 128 == 0
+    if 128 % W:
+        return False
+    rows = 128 // W
+    return rows % H == 0 if rows > H else H % rows == 0
+
+
+def diffusion_conv_planes(height: int, width: int, unet_levels: int, vae_levels: int) -> list:
+    """Every (H, W) plane on which the UNet and the VAE run `conv3x3` for images of height x width: the UNet's latent plane
+    (height / 8) halved at each of its `unet_levels` - 1 downsamples, the VAE's image plane halved at each of its `vae_levels` - 1."""
+    planes = []
+    for (h, w), levels in (((height // 8, width // 8), unet_levels), ((height, width), vae_levels)):
+        for _ in range(levels):
+            if (h, w) not in planes:
+                planes.append((h, w))
+            h, w = h // 2, w // 2
+    return planes
+
+
 def conv3x3(x_nhwc, w_k, bias=None, rowbias=None, residual=None):
     """x [N,H,W,Cin] bf16 contiguous; w_k [Cout, 9*Cin] ((r,s,c)-major); returns [N,H,W,Cout]."""
     _chk_cuda(x_nhwc, w_k, bias, rowbias, residual)
